@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — the hot path of BASELINE.json measured on B200(s).
+"""bench.py — the hot path of BASELINE.json measured on H100(s).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config c2|c3|c4|c5] [--mesh soup|grid]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
@@ -19,6 +19,9 @@ Other BASELINE configs (same JSON shape): c3 = 10M incoherent AO-style rays, any
 `--impl reference` times the reference's own CPU implementation (oracle/_ref = the unmodified reference
 compiled in place; the plain-C oracle port when that is absent) on the SAME rays with every usable host
 thread, and prints the same JSON line with "impl": "reference".
+
+`--dump-outputs DIR` writes, after the timed steps, the hit records of the last timed step as DIR/<name>.npy
+(see dump_outputs) so that two builds can be compared output for output on identical seeded inputs.
 """
 from __future__ import annotations
 
@@ -37,7 +40,7 @@ sys.path.insert(0, ROOT)
 
 from bvh_b200 import scenes  # noqa: E402
 
-FALLBACK_HBM_GBS = 6650.0        # /opt/skills/guides/B200_PROFILING.md fallback
+FALLBACK_HBM_GBS = 3350.0        # H100 SXM data sheet (HBM3), used when MEASURED_PEAKS.json is absent
 
 # BASELINE.json configs[1..4].  img: the camera is img x img primary rays; count: incoherent rays.
 CONFIGS = {
@@ -75,6 +78,8 @@ def parse_args():
                          "record — or NCCL all-gather")
     ap.add_argument("--sort-rays", action="store_true", help="BVH_SORT_RAYS: traverse the batch in the Morton order of the ray origins")
     ap.add_argument("--no-numa", action="store_true", help="N > 1: do not bind the rank to its GPU's NUMA node")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the hit records of the last timed step as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -83,7 +88,7 @@ def hbm_peak():
     try:
         return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
+        return FALLBACK_HBM_GBS, "H100 SXM data sheet"
 
 
 def usable_cpus():
@@ -112,9 +117,9 @@ def usable_cpus():
 
 
 def gather_candidates(world: int, requested: str) -> list:
-    """Delivery forms of the fused gather to try, in order; an empty list means the NCCL path.  `auto` follows the
-    measurements of DESIGN.md §7: two ranks — one multimem store per record; up to AUTO_DIRECT_MAX_RANKS — one peer store
-    per record and rank; beyond — warp-staged bulk copies, to the multicast address when the fabric has one."""
+    """Delivery forms of the fused gather to try, in order; an empty list means the NCCL path.  `auto` (DESIGN.md §7):
+    two ranks — one multimem store per record; up to AUTO_DIRECT_MAX_RANKS — one peer store per record and rank;
+    beyond — warp-staged bulk copies, to the multicast address when the fabric has one."""
     if world == 1 or requested == "nccl":
         return []
     if requested != "auto":
@@ -128,8 +133,8 @@ def gather_candidates(world: int, requested: str) -> list:
 
 def bind_to_gpu_numa_node(local_rank: int):
     """Multi-rank runs: pin this rank (and therefore the first-touch placement of its pinned host buffers)
-    to the NUMA node its GPU hangs off.  Eight ranks streaming 70 GB/s each through whatever socket the
-    scheduler put them on is what collapsed the 8-GPU e2e number in round 1."""
+    to the NUMA node its GPU hangs off: ranks streaming pinned host buffers through whichever socket the
+    scheduler put them on contend for one socket's PCIe and memory bandwidth."""
     try:
         import pynvml
         pynvml.nvmlInit()
@@ -255,6 +260,30 @@ def bytes_per_ray(cfg, s_inner, s_tri):
     if cfg["dtype"] == "f64":
         return 64 + 32 + 128 * s_inner + 96 * s_tri
     return 32 + (4 if cfg["any_hit"] else 16) + 64 * s_inner + 48 * s_tri
+
+
+DUMP_SAMPLE = 1 << 20           # hit records written by --dump-outputs (a fixed sample of larger batches)
+DUMP_SEED = 20240917
+
+
+def dump_outputs(out_dir, hits_np):
+    """Writes what the timed traversal returned in its last step: per ray the hit primitive id (float64, exact for
+    32-bit ids; -1 = miss) and t, u, v in the config's precision.  Batches above DUMP_SAMPLE rays are reduced to a
+    fixed, seeded, sorted sample of ray indices, written as ray_index.npy (float64), so the files stay under 64 MB."""
+    n = hits_np.shape[0]
+    if n > DUMP_SAMPLE:
+        index = np.sort(np.random.default_rng(DUMP_SEED).choice(n, DUMP_SAMPLE, replace=False))
+    else:
+        index = np.arange(n)
+    sel = hits_np[index]
+    ids = sel["prim_id"].astype(np.float64)
+    ids[sel["prim_id"] == np.iinfo(sel["prim_id"].dtype).max] = -1.0
+    arrays = {"ray_index": index.astype(np.float64), "prim_id": ids,
+              "t": np.ascontiguousarray(sel["t"]), "u": np.ascontiguousarray(sel["u"]), "v": np.ascontiguousarray(sel["v"])}
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    os.makedirs(out_dir, exist_ok=True)
+    for key, a in arrays.items():
+        np.save(os.path.join(out_dir, key + ".npy"), a)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -423,17 +452,12 @@ def main():
     build_e2e_ms = (time.perf_counter() - t0) / 3 * 1e3
     morton_bits = int(props.get("morton_bits", 30))
     build_bytes = 300.0 if morton_bits <= 32 else 440.0        # SURVEY.md §8(d): bytes per triangle of the LBVH pipeline
-    traffic_db = {}
-    try:
-        traffic_db = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        pass
     build_info = {"value": n_tris / build_ms / 1e3, "unit": "Mtris/s", "ms": build_ms, "steps": build_steps, "scope": "per GPU (BVH replicated)",
                   "e2e_ms_host_vertices": build_e2e_ms, "depth": bvh.depth, "morton_bits": morton_bits,
                   "quality": args.quality or "high (library default)", "pipeline": props.get("pipeline"),
                   "roofline": {"bound": "hbm", "achieved": build_bytes * n_tris / (build_ms * 1e-3) / 1e9, "peak": peak_gbs,
                                "unit": "GB/s", "frac": build_bytes * n_tris / (build_ms * 1e-3) / 1e9 / peak_gbs,
-                               "traffic": traffic_db.get(f"build_{kind}_{n_tris}"), "bytes_per_tri": build_bytes}}
+                               "bytes_per_tri": build_bytes}}
 
     # ---- algorithmic bytes of the traversal, measured on the tree actually traversed, over the WHOLE timed batch
     st = torch.empty((n_rays, 3), dtype=torch.int32, device=device)
@@ -458,10 +482,9 @@ def main():
             raise SystemExit(api.last_error())
 
     tracer, gather_desc = None, None
-    # auto: two ranks one multimem store per record (2-GPU run: 0.995 of perfect scaling, per-record peer stores 0.954, staged
-    # 0.90); up to 4 ranks one peer store per record and rank (each costs ~1-2 % of the kernel: scripts/gather_probe.py); beyond
-    # that warp-staged bulk copies (a fixed ~6 %, independent of the number of ranks) — ONE copy per 32 records to the multicast
-    # address when the fabric has one (8 ranks: 0.881), else one copy per rank (0.836); NCCL (below) if none works
+    # auto: two ranks one multimem store per record; up to 4 ranks one peer store per record and rank; beyond that
+    # warp-staged bulk copies (a cost independent of the number of ranks) — ONE copy per 32 records to the multicast
+    # address when the fabric has one, else one copy per rank; NCCL (below) if none works
     candidates = gather_candidates(world, args.gather)
     for mode in candidates:
         try:
@@ -507,8 +530,7 @@ def main():
         tracer.step()
     # Everything that can take host time (NVML initialisation of the clock sampler, event creation, a garbage collection)
     # happens BEFORE the barrier that opens the timed region: a rank that enters the region late makes every other rank
-    # wait at the first step's symmetric-memory barrier, and that wait is inside their timed window (one 87 ms step in
-    # a 20-step run halves the reported value: profiles/r02_n2_*).
+    # wait at the first step's symmetric-memory barrier, and that wait is inside their timed window.
     sampler = ClockSampler(local_rank)
     starts = [torch.cuda.Event(enable_timing=True) for _ in range(args.steps)]
     ends = [torch.cuda.Event(enable_timing=True) for _ in range(args.steps)]
@@ -547,6 +569,8 @@ def main():
         ref_sums = sums.clone()
         dist.broadcast(ref_sums, src=0)
         assert torch.equal(sums, ref_sums), "ranks disagree on the gathered hit records"
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, hits_np if world == 1 else tracer.global_hits().cpu().numpy().view(hit_dtype).reshape(-1))
 
     # ---- e2e through the C ABI with pinned host buffers ----------------------------------------------
     e2e = None
@@ -594,9 +618,8 @@ def main():
                                    "slow_steps": [[int(i), float(t)] for i, t in enumerate(step_ms) if t > 1.5 * kernel_ms]}},
             "roofline": {"bound": "hbm", "kernel": kernel_name, "achieved": achieved, "peak": peak_gbs,
                          "peak_source": peak_src, "unit": "GB/s", "frac": achieved / peak_gbs,
-                         "traffic": traffic_db.get(f"trace_{name}_{kind}"),
                          "bytes_per_ray": bpr, "launch_ms": kernel_ms,
-                         "note": "algorithmic bytes over time; the tree is L2-resident, so frac can exceed 1 (traffic = DRAM bytes per launch, ncu)"},
+                         "note": "algorithmic bytes over time; the tree is L2-resident, so frac can exceed 1"},
             "build": build_info,
             "cpu_baseline": cpu,
             "e2e": e2e,

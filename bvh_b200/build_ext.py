@@ -1,5 +1,5 @@
 """Compiles the CUDA engine into ``bvh_b200/libbvh_c.so`` (in-tree, so that it travels with the
-repository snapshot to the GPU box).  sm_100a only; nvcc cross-compiles without a GPU.
+repository tree).  sm_90a (H100) only; nvcc cross-compiles without a GPU.
 
     python -m bvh_b200.build_ext [--force] [--verbose]
 """
@@ -21,7 +21,7 @@ LIB = os.path.join(HERE, "libbvh_c" + ("_" + TAG if TAG else "") + ".so")
 
 SOURCES = ["lbvh_build.cu", "traverse.cu", "c_api.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--fmad=false",                      # parity arithmetic is written with explicit *_rn intrinsics; never contract the rest either
     "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=hidden,-Wall,-Wno-unused-function",
     "-I", os.path.join(ROOT, "include"), "-I", CSRC,
@@ -57,7 +57,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as pool:
         objs = list(pool.map(compile_one, SOURCES))
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -489,9 +489,8 @@ int intersect_batch(Handle<T>* h, const RayPod* rays, size_t n, HitPod* hits, bv
     // the staging buffers may still be in use by earlier work on the handle's stream
     BVH_CUDA_TRY(cudaEventRecord(h->events[0], h->stream));
     BVH_CUDA_TRY(cudaStreamWaitEvent(h->copy_in, h->events[0], 0));
-    // Equal chunks.  Measured (profiles/r01_e2e_chunking.txt): 8 equal chunks 6.86 ms; with chunk sizes tapering
-    // towards the end 7.12 ms (and 7.43 / 6.96 / 7.37 ms for 6 / 12 / 16 tapered chunks).  Upload (320 MB) and
-    // download (160 MB) share the link: the call runs at ~70 GB/s of combined PCIe traffic whatever the schedule.
+    // Equal chunks (chunk sizes tapering towards the end were no faster on an earlier GPU).  Upload and download share
+    // the PCIe link: the call is bound by the combined copy traffic whatever the schedule.
     for (size_t c = 0; c < chunks; ++c) {
         const size_t b = n * c / chunks, e = n * (c + 1) / chunks;
         cudaEvent_t in_done = h->events[1 + 2 * c], tr_done = h->events[2 + 2 * c];

@@ -105,11 +105,9 @@ static_assert(sizeof(DevNode<float>) == 32 && sizeof(DevNode<double>) == 64, "pa
 
 // reference tri.h:30-37 (PrecomputedTri): p0, e1 = p0-p1, e2 = p2-p0, n = cross(e1, e2)
 // PrecomputedTri (tri.h:30-37), packed: 48 / 96 bytes, three / six 128-bit loads per test.  The padded form (BVH_TRI_PAD:
-// 64 / 128 bytes, two / three 256-bit loads) was measured on the B200 and is no faster: soup-1M 3057 vs 3083 Mrays/s packed,
-// grid 6178 vs 6233, c3 1670 vs 1661 (profiles/r02_run8_ab.txt) — the wavefronts it saves are paid back by the L2 hit rate
-// (94.2 % -> 91.9 %: 16 MB more footprint per million triangles next to 480 MB of streamed rays and hits).
+// 64 / 128 bytes, four / eight 128-bit loads) costs 16 MB more footprint per million triangles; not measured on the H100.
 #ifndef BVH_TRI_PAD
-#define BVH_TRI_PAD 0              // 1: 64 / 128-byte records, two / three 256-bit loads per test (measured: no faster, see below)
+#define BVH_TRI_PAD 0              // 1: 64 / 128-byte records
 #endif
 #if BVH_TRI_PAD
 template <typename T> struct alignas(16 * sizeof(T)) DevTri { T p0[3], e1[3], e2[3], n[3], pad[4]; };

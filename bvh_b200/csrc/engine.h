@@ -34,7 +34,7 @@ int device_alloc(void** ptr, size_t bytes, cudaStream_t stream);
 void device_free(void* ptr, cudaStream_t stream);
 int prepare_device(int device);
 
-// Process-wide switches for experiments and tests; the defaults are the measured best.  Initialised once from
+// Process-wide switches for experiments and tests; the defaults are the tuned values.  Initialised once from
 // the BVH_B200_* environment variables (DESIGN.md), changed at run time with bvh_set_option — nothing on a
 // call path reads the environment.
 struct Tunables {

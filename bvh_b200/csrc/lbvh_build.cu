@@ -1,4 +1,4 @@
-// bvh_b200/csrc/lbvh_build.cu — the CUDA LBVH construction pipeline (sm_100a).
+// bvh_b200/csrc/lbvh_build.cu — the CUDA LBVH construction pipeline (sm_90a).
 //
 // Replaces DefaultBuilder<Node>::build (reference default_builder.h:33-62) and everything under it.
 // Kernels, in launch order (DESIGN.md has the byte accounting):
@@ -250,9 +250,8 @@ hierarchy_thread_kernel(BuildParams<T> p, const K* __restrict__ keys, const uint
     climb_global<T, K, DeviceSync>(p, keys, st, parent, side, published_record(st));
 }
 
-// Variant selection.  Measured on B200 (1M-triangle soup, whole build, median of 25; profiles/r01_build_variants.txt):
-// global 313 us, thread64 301, thread128 303, thread256 314-320 — the pass is bound by the dependent chain of the
-// top levels and the vertex gather of the leaf stage, which all variants share, so the spread is small.
+// Variant selection.  The pass is bound by the dependent chain of the top levels and the vertex gather of the leaf
+// stage, which all variants share, so they differ little; thread128 is the default (not re-measured on the H100).
 // BVH_B200_HIERARCHY=global|thread64|thread128|thread256 overrides the default for experiments; all variants
 // build the same tree (tests/test_host_emulation.py::test_block_local_phase_builds_the_same_tree).
 template <typename T, typename K>
@@ -559,8 +558,8 @@ int build_wide(DeviceBvh<float>& bvh, uint32_t levels, uint32_t* d_counters, uin
     if (!bvh.wide && device_alloc(reinterpret_cast<void**>(&bvh.wide), (size_t)(n ? n : 1) * sizeof(WideNode), stream)) return -1;
     wide_init_kernel<<<1, 64, 0, stream>>>(d_frontier_a, d_counters);
     if (levels > (uint32_t)kWideMaxLevels) levels = kWideMaxLevels;
-    // One launch per level.  (Measured and removed, round 2: all levels in one cooperative launch with a grid-wide
-    // barrier per level — 447 us per million triangles against 280 us for these ~25 small launches.)
+    // One launch per level.  (All levels in one cooperative launch with a grid-wide barrier per level was slower than
+    // these ~25 small launches on an earlier GPU and was removed.)
     uint64_t bound = 1;
     for (uint32_t level = 0; level < levels; ++level) {
         const uint64_t items = bound < n ? bound : n;                     // frontier L has at most min(4^L, n) items
@@ -634,7 +633,7 @@ int build_with_key(DeviceBvh<T>& out, const T* d_verts, const T* d_bboxes, const
     const T* centre_src = d_verts ? d_verts : d_centers;
     const T* leaf_src = d_verts ? d_verts : d_bboxes;
 
-    int sm_count = 148;
+    int sm_count = 132;
     cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, out.device);
     const uint32_t blocks_needed = (n + kBlock - 1) / kBlock;
     const uint32_t grid = blocks_needed < (uint32_t)(sm_count * 4) ? blocks_needed : (uint32_t)(sm_count * 4);

@@ -256,7 +256,7 @@ rs_onesweep_kernel(const K* __restrict__ keys_in, const uint32_t* __restrict__ v
             // Look back in windows of kOsWindow descriptors: the loads of a window are independent (all in flight at
             // once), then the window is consumed nearest first.  With every tile of a pass resident at the same time
             // most predecessors still show an AGGREGATE when a tile starts to look, so the walk is long; one load per
-            // step made a pass no faster than the three-kernel form (29 us per million keys, profiles/r02_*launches*).
+            // step made a pass no faster than the three-kernel form.
             bool done = false;
             for (uint32_t hi = tile; hi > 0 && !done;) {                   // predecessors hi-1, hi-2, ...
                 const uint32_t span = hi < (uint32_t)kOsWindow ? hi : (uint32_t)kOsWindow;

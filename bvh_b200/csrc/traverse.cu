@@ -1,4 +1,4 @@
-// bvh_b200/csrc/traverse.cu — batched closest-hit / any-hit ray traversal kernels (sm_100a).
+// bvh_b200/csrc/traverse.cu — batched closest-hit / any-hit ray traversal kernels (sm_90a).
 //
 // Replaces the caller-side ray loop around Bvh::intersect (reference bvh.h:159-182 driven by
 // test/benchmark.cpp:340-393 / c_api/bvh_impl.h:235-250) with two kernels over a whole ray batch:
@@ -34,10 +34,9 @@ namespace bvhb200 {
 namespace {
 
 // Resident blocks per SM the persistent kernel's registers are limited for (float, the variants without hit staging):
-// 8 -> 64 registers, 9 -> 56 (10 / 12 bytes of spills), 10 -> 48 (34 / 28 bytes).  Measured on the B200 (profiles/
-// r02_run15_occupancy_ab.txt): soup-1M 3522 / 3665 / 3658 Mrays/s, grid-1M 6552 / 6794 / 6807, c3 1901 / 1973 / 1955 — the
-// final-state kernel saturates no pipe (L1 74 %, issue 70 %), so four more warps per SM to hide latency pay.  The variants
-// with warp-staged hit stores (kGather) keep 8: that is the form the 8-GPU runs measured.
+// 8 -> 64 registers, 9 -> 56, 10 -> 48.  The kernel is latency-bound, so more resident warps per SM hide more of it; on
+// the H100 (bench.py c2 / c3) 12 blocks (40 registers, spills) were measured 1.4x slower than 9.  The variants with
+// warp-staged hit stores (kGather) keep 8.
 #ifndef BVH_TRACE_BLOCKS
 #define BVH_TRACE_BLOCKS 9
 #endif
@@ -519,8 +518,7 @@ trace_persistent_kernel(TraceArgs<T> a) {
         // A warp draws new rays only once refill_min of its lanes are idle.  The rays drawn together are neighbours
         // (consecutive indices of one chunk) and start at the root in the same iteration, so they stay in step through
         // the top of the tree and their node fetches — same address in the same instruction — cost one L1 wavefront
-        // instead of one per lane; the price is idle lanes, which this L1-bound kernel can afford (measured on the B200,
-        // profiles/r02_run5_*: soup-1M 2806 -> 3082 Mrays/s at 8, grid-1M 5959 -> 6530 at 20; 32 = no refill: 2270).
+        // instead of one per lane; the price is idle lanes, which this L1-bound kernel can afford.
         unsigned idle = __ballot_sync(kFull, !has_ray);
         if ((uint32_t)__popc(idle) < a.refill_min) idle = 0u;
         while (idle != 0u && !exhausted) {
@@ -641,8 +639,8 @@ trace_pair_kernel(TraceArgs<T> a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     // The member mask of every warp-synchronous primitive below comes from a kernel argument (always
     // 0xFFFFFFFF).  With a compile-time full mask ptxas elides the hardware warp barrier wherever it
-    // believes the warp is already converged and keeps the round counter in a uniform register; on B200
-    // that produced occasional hangs of this kernel (a warp split in two that never rejoined, found with
+    // believes the warp is already converged and keeps the round counter in a uniform register; on an
+    // earlier GPU that produced occasional hangs of this kernel (a warp split in two that never rejoined, found with
     // the watchdog below).  A run-time mask forces a real WARPSYNC in front of each vote / shuffle.
     const unsigned kFull = a.full_mask;
     constexpr unsigned kEven = 0x55555555u;
@@ -848,9 +846,8 @@ trace_wide_kernel(TraceArgs<float> a) {
         }
 
         // ---- inner phase ----------------------------------------------------------------------------
-        // (Measured and removed, round 2: speculative descent — a lane that reaches a leaf puts it aside once and
-        // keeps descending — 2.69 instead of 2.77 Grays/s on soup-1M, 4.82 instead of 5.16 on grid-1M: the steps taken
-        // before tmax shrinks cost more than the idle lanes they fill.)
+        // (Speculative descent — a lane that reaches a leaf puts it aside once and keeps descending — was measured
+        // slower on an earlier GPU and removed: the steps taken before tmax shrinks cost more than the idle lanes they fill.)
         if (has_ray) {
             uint32_t budget = inner_budget;
             while (index_count(top) == 0 && budget != 0) {
@@ -859,8 +856,8 @@ trace_wide_kernel(TraceArgs<float> a) {
                 {
                     uint32_t w0[8], w1[8];
                     const WideNode* node = a.wide + (top >> kPrimCountBits);
-                    ldg256(node, w0);                       // (allocating: a wide node serves four children; no_allocate
-                    ldg256(reinterpret_cast<const unsigned char*>(node) + 32, w1);      //  measured -10 % on incoherent rays here)
+                    ldg256(node, w0);                       // (allocating: a wide node serves four children)
+                    ldg256(reinterpret_cast<const unsigned char*>(node) + 32, w1);
                     #pragma unroll
                     for (int k = 0; k < 8; ++k) { w[k] = w0[k]; w[8 + k] = w1[k]; }
                 }
@@ -941,7 +938,7 @@ int make_ray_order(const DeviceBvh<T>& bvh, const DevRay<T>* d_rays, uint32_t n,
     uint32_t* vals_a = static_cast<uint32_t*>(scratch.ptrs[2]); uint32_t* vals_b = static_cast<uint32_t*>(scratch.ptrs[3]);
     uint32_t* state = static_cast<uint32_t*>(scratch.ptrs[4]);
     BVH_CUDA_TRY(cudaMemsetAsync(state, 0, words * sizeof(uint32_t), stream));
-    int sm_count = 148;
+    int sm_count = 132;
     BVH_CUDA_TRY(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, bvh.device));
     const uint32_t want = (n + 255) / 256, cap = (uint32_t)sm_count * 4;
     ray_key_kernel<T><<<want < cap ? want : cap, 256, 0, stream>>>(d_rays, n, bvh.nodes, keys_a, state + 64);
@@ -959,14 +956,14 @@ int configure_smem(KernelT kernel, size_t smem_bytes) {
     return 0;
 }
 
-// One resident wave of persistent CTAs (148 SMs x occupancy), never more than the batch can feed.
+// One resident wave of persistent CTAs (SM count x occupancy), never more than the batch can feed.
 template <typename KernelT, typename T>
 int launch_persistent(KernelT kernel, const TraceArgs<T>& args, size_t smem, unsigned rays_per_warp, int device, cudaStream_t stream) {
     if (smem > 200 * 1024) { set_error("trace: tree too deep for the shared-memory stack"); return -1; }
     if (configure_smem(kernel, smem)) return -1;
     if (const int carve = tunables().smem_carveout.load(); carve >= 0)
         BVH_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve));
-    int sm_count = 148, per_sm = 1;
+    int sm_count = 132, per_sm = 1;
     BVH_CUDA_TRY(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device));
     BVH_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kTraceBlock, smem));
     if (per_sm < 1) per_sm = 1;
@@ -1057,7 +1054,9 @@ int trace_rays(const DeviceBvh<T>& bvh, const DevRay<T>* d_rays, DevHit<T>* d_hi
     args.refill_min = tunables().refill_min.load();
     {   // a warp's private run of consecutive rays: as long as the batch allows with ~8 runs per resident warp (tail balance)
         uint32_t run = tunables().chunk_rays.load();
-        const unsigned long long fair = n / (148ull * 32ull * 8ull);
+        int sm_count = 132;
+        BVH_CUDA_TRY(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, bvh.device));
+        const unsigned long long fair = n / ((unsigned long long)sm_count * 32ull * 8ull);
         if (fair < run) run = (uint32_t)fair;
         run &= ~31u;
         args.chunk_rays = run < 32u ? 32u : run;

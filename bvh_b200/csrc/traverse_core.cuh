@@ -22,22 +22,26 @@ template <typename T> struct NodePair {
 };
 
 #if defined(__CUDACC__)
+// 32 bytes as two 128-bit loads from one 32-byte aligned block: sm_90 has no 256-bit global load, and the widest
+// vector load it has (LDG.E.128) keeps both halves in the same L1 sector pair.
 __device__ __forceinline__ void ldg256(const void* p, uint32_t (&w)[8]) {
-    asm("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+        "ld.global.nc.v4.b32 {%4,%5,%6,%7}, [%8+16];"
         : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
 }
-// Node loads do NOT allocate their line in L1 (ld.global.nc.L1::no_allocate).  Measured on the B200 (profiles/
-// r02_run10to11_*): soup-1M +6.4 %, incoherent c3 +8 %, grid-1M -0.5 %.  Deep nodes are used once per ray, and a pending miss
-// that must allocate a line is limited by the L1's capacity: with 28 KB of L1 (the 228 KB shared-memory carve-out) the
-// incoherent batch ran at 1.0 instead of 1.7 Grays/s — the lines in flight, not the hits, were what the larger L1 bought.
+// Node loads allocate their line in L1 (BVH_NODE_NA=0).  Measured on an H100 80GB HBM3 SXM at a 400 W power limit
+// (bench.py, 1M-triangle soup, 10M rays): allocating loads take 4.09 instead of 6.96 ms per step for coherent primary
+// rays and 11.0 instead of 23.1 ms for incoherent any-hit rays; BVH_NODE_NA=1 (ld.global.nc.L1::no_allocate) keeps the
+// other form selectable.
 #ifndef BVH_NODE_NA
-#define BVH_NODE_NA 1
+#define BVH_NODE_NA 0
 #endif
 #ifndef BVH_TRI_NA
 #define BVH_TRI_NA 0
 #endif
 __device__ __forceinline__ void ldg256_na(const void* p, uint32_t (&w)[8]) {
-    asm("ld.global.nc.L1::no_allocate.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm("ld.global.nc.L1::no_allocate.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+        "ld.global.nc.L1::no_allocate.v4.b32 {%4,%5,%6,%7}, [%8+16];"
         : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
 }
 __device__ __forceinline__ void ldg256_node(const void* p, uint32_t (&w)[8]) {
@@ -57,11 +61,13 @@ __device__ __forceinline__ float4 ldg128_tri(const float4* p) {
 #endif
 }
 __device__ __forceinline__ void ldg256(const void* p, unsigned long long (&w)[4]) {
-    asm("ld.global.nc.v4.b64 {%0,%1,%2,%3}, [%4];" : "=l"(w[0]), "=l"(w[1]), "=l"(w[2]), "=l"(w[3]) : "l"(p));
+    asm("ld.global.nc.v2.b64 {%0,%1}, [%4];\n\t"
+        "ld.global.nc.v2.b64 {%2,%3}, [%4+16];" : "=l"(w[0]), "=l"(w[1]), "=l"(w[2]), "=l"(w[3]) : "l"(p));
 }
 __device__ __forceinline__ void ldg256_node(const void* p, unsigned long long (&w)[4]) {
 #if BVH_NODE_NA
-    asm("ld.global.nc.L1::no_allocate.v4.b64 {%0,%1,%2,%3}, [%4];" : "=l"(w[0]), "=l"(w[1]), "=l"(w[2]), "=l"(w[3]) : "l"(p));
+    asm("ld.global.nc.L1::no_allocate.v2.b64 {%0,%1}, [%4];\n\t"
+        "ld.global.nc.L1::no_allocate.v2.b64 {%2,%3}, [%4+16];" : "=l"(w[0]), "=l"(w[1]), "=l"(w[2]), "=l"(w[3]) : "l"(p));
 #else
     ldg256(p, w);
 #endif

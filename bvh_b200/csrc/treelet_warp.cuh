@@ -22,8 +22,8 @@
 // aggregates with warp shuffles, and the carry-in; the stable partition ranks a position with two ballots and
 // population counts.  Shared memory (3.3 KB per warp for float) only holds what is indexed by PRIMITIVE or read
 // from another lane's position: the primitive boxes, the three orders, per-head decisions.  (The first version of
-// this pass kept every per-position array in shared memory and ran ~600 __syncwarp-separated phases per treelet:
-// 1.88 ms per million triangles on the B200, profiles/r02_*; this one needs about a tenth of the instructions.)
+// this pass kept every per-position array in shared memory and ran ~600 __syncwarp-separated phases per treelet;
+// this one needs about a tenth of the instructions.)
 //
 // The algorithm is written ONCE against a lane-execution policy: on the device a per-lane variable is a register
 // and `each` runs the body for the calling lane; in the host emulation (tests/host_emul.cpp) a per-lane variable

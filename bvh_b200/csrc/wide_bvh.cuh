@@ -152,13 +152,9 @@ BVH_HD float wide_fmin(float a, float b) {
 #endif
 }
 
-// Byte c of a packed word as a float: a plain int-to-float conversion (I2F, on the XU pipe).  Measured alternatives:
-// round 1 — one PRMT dropping the byte into the mantissa of 2^23 plus an exact subtraction: XU 80 % -> 6 % of peak
-// but an extra issue slot per value, 2.68-2.72 instead of 3.00 Grays/s; round 2 — the same permute with the offset
-// folded into the per-node constant (t = fma(32768 + q, s, b - 32768 s), b rounded outwards), no extra instruction
-// per value: XU 6 %, but the permutes land on the ALU pipe, which also carries the kernel's min/max, compares and
-// selects (ALU 67 % of peak, issue 82 %, profiles/r02_wide_prmt_soup1M.txt): 2.67 Grays/s on the tree round 1 traced
-// at 3.0.  The conversions stay on the XU pipe, which nothing else in this kernel uses.
+// Byte c of a packed word as a float: a plain int-to-float conversion (I2F, on the XU pipe, which nothing else in this
+// kernel uses).  Byte permutes into the mantissa of a power of two were measured slower on an earlier GPU: they cost an
+// extra issue slot per value or load the ALU pipe that also carries the kernel's min/max, compares and selects.
 BVH_HD float wide_byte_to_float(uint32_t word, int c) { return (float)((word >> (8 * c)) & 0xFFu); }
 
 // One inner step through the wide node whose 16 words are in w (layout of WideNode).  Dequantises the four

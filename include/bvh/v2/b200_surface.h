@@ -1,4 +1,4 @@
-// include/bvh/v2/b200_surface.h — the reference library's C++ API surface on top of the B200 engine.
+// include/bvh/v2/b200_surface.h — the reference library's C++ API surface on top of the CUDA engine.
 //
 // The reference is header-only C++20 templates (reference src/bvh/v2/*.h).  Its users write
 //     bvh::v2::DefaultBuilder<Node>::build(thread_pool, bboxes, centers, config)   (default_builder.h:33-62)

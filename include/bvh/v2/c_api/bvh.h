@@ -1,4 +1,4 @@
-/* include/bvh/v2/c_api/bvh.h — the reference library's C API surface, re-declared for the B200 engine.
+/* include/bvh/v2/c_api/bvh.h — the reference library's C API surface, re-declared for the CUDA engine.
  *
  * Same include path, names, signatures and POD layouts as the reference header
  * (reference src/bvh/v2/c_api/bvh.h:32-295), so C callers written against the reference

@@ -1,4 +1,4 @@
-/* include/bvh_b200.h — C ABI of the B200-native BVH engine (libbvh_c.so).
+/* include/bvh_b200.h — C ABI of the H100-native BVH engine (libbvh_c.so).
  *
  * Two groups of entry points, all `extern "C"`, plain pointers and sizes:
  *

@@ -3,7 +3,7 @@
 dram__bytes_write.sum): per kernel count, mean / min / max duration and DRAM bytes per launch, plus the totals of ONE
 build (centre_bounds_kernel .. the last build kernel before the next build or the first traversal).
 
-    python scripts/summarize_launches.py gpurun_out/launches.csv [--traffic profiles/traffic.json --key build_soup_1000000]
+    python scripts/summarize_launches.py launches.csv [--traffic traffic.json --key build_soup_1000000]
 """
 import argparse
 import collections

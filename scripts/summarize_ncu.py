@@ -1,7 +1,7 @@
-"""Summarises an .ncu-rep (captured on the GPU box with `ncu --set full`) into a small text file for
-profiles/: one block per kernel launch with the metrics DESIGN.md / bench.py refer to.
+"""Summarises an .ncu-rep (captured with `ncu --set full`) into a small text file: one block per kernel launch
+with the metrics DESIGN.md / bench.py refer to.
 
-    python scripts/summarize_ncu.py gpurun_out/prof.ncu-rep profiles/r01_xxx.txt ["free-text note"]
+    python scripts/summarize_ncu.py prof.ncu-rep summary.txt ["free-text note"]
 """
 import csv
 import io

@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with `-m gpu`)")
 
 
 @pytest.fixture(scope="session")
@@ -25,7 +25,7 @@ def oracle():
 def ref():
     from oracle.pyoracle import Ref, ref_available
     if not ref_available():
-        pytest.skip("oracle/_ref/libbvh_ref.so not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/libbvh_ref.so not built (needs BVH_REFERENCE_DIR at build time)")
     return Ref()
 
 
@@ -44,5 +44,5 @@ def gpu_lib():
     """The CUDA library with a visible device; GPU tests fail loudly when either is missing."""
     import bvh_b200.api as api
     api.lib()
-    assert api.device_count() > 0, "no CUDA device visible: GPU tests must run on the B200 box"
+    assert api.device_count() > 0, "no CUDA device visible: GPU tests must run on an H100"
     return api

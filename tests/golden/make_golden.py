@@ -1,7 +1,7 @@
-"""Generates the committed golden vectors from the UNMODIFIED reference (oracle/_ref/libbvh_ref.so,
-i.e. /root/reference compiled in place).  Run in the build container only:
+"""Generates the committed golden vectors from the UNMODIFIED reference (oracle/_ref/libbvh_ref.so, built by
+__graft_entry__.build() when BVH_REFERENCE_DIR names a checkout of madmann91/bvh):
 
-    python tests/golden/make_golden.py
+    BVH_REFERENCE_DIR=<checkout> python tests/golden/make_golden.py
 
 Outputs (small .npz files next to this script):
   kat_simple_example.npz   reference test/simple_example.cpp: 2 triangles, 1 ray -> prim 1 (BVH order), t=1, u=-0, v=0.5
@@ -83,7 +83,7 @@ blob = ref.serialize(tree2)
 np.savez(os.path.join(OUT, "kat_serialize.npz"), tris=two, bboxes=bb, centers=cc, blob=np.frombuffer(blob, np.uint8))
 print("serialize:", len(blob), "bytes", blob.hex())
 
-cornell = load_obj_tris("/root/reference/test/scenes/cornell_box.obj")
+cornell = load_obj_tris(os.path.join(os.environ["BVH_REFERENCE_DIR"], "test", "scenes", "cornell_box.obj"))
 bb, cc = ref.tri_bboxes_centers(cornell)
 tree = ref.build(bb, cc, quality="high", threads=0)
 ref.set_triangles(tree, cornell)

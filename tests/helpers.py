@@ -1,5 +1,7 @@
 """Test helpers: the host emulation of the device code (tests/host_emul.cpp) and comparison utilities."""
 import ctypes as C
+import hashlib
+import json
 import os
 import subprocess
 
@@ -183,3 +185,40 @@ def assert_hits_conservative(got, want, tris, rays, oracle, what="", max_fractio
         assert g[1][i] < want[1][i] or (g[1][i] == want[1][i] and g[0][i] < want[0][i]), f"{what}: ray {i} is not closer"
         one = oracle.brute_force(tris[int(g[0][i]):int(g[0][i]) + 1], rays[i:i + 1])
         assert one[0][0] == 0 and one[1][0] == g[1][i] and one[2][0] == g[2][i] and one[3][0] == g[3][i], f"{what}: ray {i}: not a real hit"
+
+
+def digest(a) -> str:
+    """SHA-256 of an array's dtype, shape and bytes: the stored form of an output of the original project that a test
+    compares with bit for bit (tests/golden/reference_digests.json, written by tests/golden/make_reference_digests.py)."""
+    a = np.ascontiguousarray(a)
+    h = hashlib.sha256(f"{a.dtype.str}{a.shape}".encode())
+    h.update(a.tobytes())
+    return h.hexdigest()
+
+
+def reference_digests(section):
+    with open(os.path.join(ROOT, "tests", "golden", "reference_digests.json")) as f:
+        return json.load(f)[section]
+
+
+def reference_tree(key, boxes, dim, dtype):
+    """The serialised bytes (bvh.h:220-242) of a tree the original project built over `boxes` ([min..., max...] per
+    primitive), rebuilt from its stored topology (tests/golden/reference_trees.npz: node index words and primitive
+    order).  Node boxes are unions of primitive boxes, which min / max compute exactly, so the bytes are the original's."""
+    g = np.load(os.path.join(ROOT, "tests", "golden", "reference_trees.npz"))
+    index, ids = g[key + "_index"], g[key + "_ids"]
+    it = np.uint32 if dtype == np.float32 else np.uint64
+    lo, hi = boxes[:, :dim], boxes[:, dim:]
+    bounds = np.empty((index.shape[0], 2 * dim), dtype)
+    for i in range(index.shape[0] - 1, -1, -1):                  # children come after their parent
+        count, first = int(index[i] & 15), int(index[i] >> 4)
+        if count:
+            sel = ids[first:first + count]
+            bounds[i, 0::2], bounds[i, 1::2] = lo[sel].min(axis=0), hi[sel].max(axis=0)
+        else:
+            c = bounds[first:first + 2]
+            bounds[i, 0::2], bounds[i, 1::2] = c[:, 0::2].min(axis=0), c[:, 1::2].max(axis=0)
+    node_dt = np.dtype([("bounds", dtype, 2 * dim), ("index", it)])
+    nodes = np.empty(index.shape[0], node_dt)
+    nodes["bounds"], nodes["index"] = bounds, index
+    return np.array([index.shape[0], ids.shape[0]], it).tobytes() + nodes.tobytes() + ids.astype(it).tobytes()
