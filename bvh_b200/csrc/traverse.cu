@@ -52,7 +52,7 @@ template <typename U> struct SmemStack {
     uint32_t top;                                            // shared-window address of the next free entry
     uint32_t step;                                           // bytes between entries
     U* base;
-    static constexpr U kSentinel = (U)~(U)0;
+    static constexpr U kSentinel = kTraversalDone<U>;
     __device__ __forceinline__ SmemStack(U* base_, uint32_t stride, uint32_t) : step(stride * (uint32_t)sizeof(U)), base(base_) {
         clear();
         top -= step;
@@ -594,11 +594,14 @@ trace_persistent_kernel(TraceArgs<T> a) {
         //      budget of this round is spent (bounding the wait of lanes that already hold a leaf) ----
         if (has_ray) {
             uint32_t budget = inner_budget;
-            while (index_count(top) == 0 && budget != 0) {
+            while (index_count(top) == 0 && budget != 0) {                     // (kTraversalDone ends it too)
                 --budget;
-                if (!inner_step<T, kAny, kRobust>(a.nodes, r, top, stack)) { has_ray = false; break; }
+                inner_step<T, kAny, kRobust>(a.nodes, r, top, stack);
             }
-            if (!has_ray) retire(ray_index, hit, tmax_in);
+            if (top == kTraversalDone<U>) {
+                retire(ray_index, hit, tmax_in);
+                has_ray = false;
+            }
         }
         __syncwarp();
 

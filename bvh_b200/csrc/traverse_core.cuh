@@ -157,14 +157,30 @@ template <typename T> inline void load_pair(const DevNode<T>* p, NodePair<T>& o)
 template <typename T> inline void load_tri(const DevTri<T>* p, DevTri<T>& o) { o = *p; }
 #endif
 
-// One inner step (reference bvh.h:132-150 with the lambda of :167-181).  Returns false when both
-// children were missed and the stack is empty, i.e. the traversal is over.
+// The value `top` takes when a ray's traversal is over: all ones, a leaf of 15 primitives at the last representable
+// position, which no tree has.  Its primitive count is not 0, so the inner-node loops stop on it without a test of their
+// own, and the ray's end needs no flag beside `top`.
+template <typename U> constexpr U kTraversalDone = (U)~(U)0;
+
+// The next entry of the stack, or kTraversalDone when it is empty.  The device stack keeps kTraversalDone in its bottom
+// entry (SmemStack, traverse.cu), so there the result is the loaded value itself (the compare only keeps the stack
+// pointer at the bottom).
+template <typename U, typename Stack> BVH_HD U pop_or_done(Stack& stack) {
+    U v = kTraversalDone<U>;
+    return stack.try_pop(v) ? v : kTraversalDone<U>;
+}
+
+// One inner step (reference bvh.h:132-150 with the lambda of :167-181): `top` (an inner node) becomes the next node to
+// visit, or kTraversalDone when both children were missed and the stack is empty.
 template <typename T, bool kAny, bool kRobust, typename Stack>
-BVH_HD bool inner_step(const DevNode<T>* __restrict__ nodes, const RayCtx<T>& r,
+BVH_HD void inner_step(const DevNode<T>* __restrict__ nodes, const RayCtx<T>& r,
                        typename Real<T>::UInt& top, Stack& stack) {
     using U = typename Real<T>::UInt;
     NodePair<T> pair;
-    load_pair(nodes + (size_t)index_first(top) + 1, pair);      // device slot = reference index + 1
+    // Device slot = reference index + 1.  An inner node's count bits are 0, so its first child's byte offset is
+    // index_first(top) * sizeof(DevNode<T>) = top * (sizeof(DevNode<T>) >> kPrimCountBits): one multiply-add from `top`.
+    load_pair(reinterpret_cast<const DevNode<T>*>(reinterpret_cast<const unsigned char*>(nodes + 1) +
+                                                  (size_t)top * (sizeof(DevNode<T>) >> kPrimCountBits)), pair);
     T l0, l1, r0, r1;
     node_test<T, kRobust>(pair.lb, r, l0, l1);
     node_test<T, kRobust>(pair.rb, r, r0, r1);
@@ -176,8 +192,7 @@ BVH_HD bool inner_step(const DevNode<T>* __restrict__ nodes, const RayCtx<T>& r,
     const U near_index = (hit_left && !right_first) ? pair.li : pair.ri;
     const U far_index = right_first ? pair.li : pair.ri;
     if (both) stack.push(far_index);
-    if (hit_left || hit_right) { top = near_index; return true; }
-    return stack.try_pop(top);
+    top = (hit_left || hit_right) ? near_index : pop_or_done<U>(stack);
 }
 
 // Leaf processing (benchmark.cpp:281-292).  stats (nullable): [1] leaves, [2] triangle tests.
@@ -199,18 +214,18 @@ template <typename T, bool kAny, bool kRobust, typename Stack>
 BVH_HD void traverse_ray(const DevNode<T>* __restrict__ nodes, const DevTri<T>* __restrict__ tris,
                          const uint32_t* __restrict__ prim_ids, bool lowest_id, typename Real<T>::UInt root_index,
                          RayCtx<T>& r, HitState<T>& hit, Stack& stack, uint32_t* stats) {
+    using U = typename Real<T>::UInt;
     if (ray_interval_is_nan(r)) return;                         // can never hit (node.h:110-115, tri.h:69)
-    typename Real<T>::UInt top = root_index;                    // get_root().index, bvh.h:54
+    U top = root_index;                                         // get_root().index, bvh.h:54
     for (;;) {
-        bool alive = true;
         while (index_count(top) == 0) {
             if (stats) stats[0] += 1;
-            if (!inner_step<T, kAny, kRobust>(nodes, r, top, stack)) { alive = false; break; }
+            inner_step<T, kAny, kRobust>(nodes, r, top, stack);
         }
-        if (!alive) break;
+        if (top == kTraversalDone<U>) break;
         leaf_step<T>(tris, prim_ids, lowest_id, top, r, hit, stats);
         if (kAny && hit.slot != kInvalidId) break;              // bvh.h:153-155
-        if (!stack.try_pop(top)) break;
+        top = pop_or_done<U>(stack);
     }
 }
 
