@@ -42,6 +42,12 @@ class BuildConfig(C.Structure):
                 ("parallel_threshold", C.c_size_t)]
 
 
+class DeviceView(C.Structure):
+    """``struct bvh_device_view3f`` / ``bvh_device_view3d`` (include/bvh_b200.h): the same layout for both."""
+    _fields_ = [("device", C.c_int), ("stream", C.c_void_p), ("nodes", C.c_void_p), ("prim_ids", C.c_void_p),
+                ("tris", C.c_void_p), ("node_count", C.c_size_t), ("prim_count", C.c_size_t), ("depth", C.c_size_t)]
+
+
 class BvhError(RuntimeError):
     pass
 
@@ -111,6 +117,8 @@ def lib() -> C.CDLL:
         f("get_property").argtypes = [P, C.c_int]
         f("get_prim_ids").restype = P
         f("get_prim_ids").argtypes = [P]
+        f("get_device_view").restype = C.c_int
+        f("get_device_view").argtypes = [P, C.POINTER(DeviceView)]
         for name in ("intersect_ray", "intersect_ray_any", "intersect_ray_robust", "intersect_ray_any_robust"):
             f(name).argtypes = [P, P, P]
         n = lambda name: getattr(L, f"bvh_node{s}_{name}")
@@ -290,6 +298,16 @@ class Bvh:
     def sync(self) -> None:
         if self._f("sync")(self.handle):
             raise BvhError(last_error())
+
+    def device_view(self) -> dict:
+        """``bvhNN_get_device_view``: the device tree for CUDA kernels of your own (include/bvh/v2/cuda/intersect.cuh), as
+        ints: device, stream, the device addresses nodes / prim_ids / tris (0 without triangles), node_count,
+        prim_count and depth.  The addresses stay valid until the tree is rebuilt, re-uploaded after a mirror edit or
+        destroyed, and tris until set_triangles."""
+        v = DeviceView()
+        if self._f("get_device_view")(self.handle, C.byref(v)):
+            raise BvhError(last_error())
+        return {name: int(getattr(v, name) or 0) for name, _ in DeviceView._fields_}
 
     # -- reference-style introspection (host mirror) -------------------------------------------
     @property

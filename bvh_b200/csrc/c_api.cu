@@ -10,6 +10,7 @@
 // edited through bvhNN_get_node / bvhNN_load is re-uploaded before the next batched call.
 #define BVH_BUILD_API
 #include <bvh_b200.h>
+#include <bvh_b200_device.h>
 
 #include <algorithm>
 #include <cstdio>
@@ -888,6 +889,24 @@ BVH_EXPORT void bvh_thread_pool_destroy(struct bvh_thread_pool* pool) { delete p
             case BVH_PROP_STREAM: return (size_t)reinterpret_cast<uintptr_t>(h->stream);                           \
             default: return (size_t)-1;                                                                            \
         }                                                                                                          \
+    }                                                                                                              \
+    BVH_EXPORT int bvh##S##_get_device_view(struct bvh##S* bvh, struct bvh_device_view##S* view) {                 \
+        auto h = H(T, bvh);                                                                                        \
+        if (!h) { set_error("get_device_view: null handle"); return -1; }                                          \
+        if (!view) { set_error("get_device_view: null view"); return -1; }                                         \
+        std::lock_guard<std::mutex> lock(h->batch_mutex);                                                          \
+        BVH_ON_DEVICE(h->device);                                                                                  \
+        if (ensure_device(*h)) return -1;                                                                          \
+        if (!h->dev.nodes || h->dev.node_slots < 2) { set_error("get_device_view: handle holds no BVH"); return -1; } \
+        view->device = h->device;                                                                                  \
+        view->stream = h->stream;                                                                                  \
+        view->nodes = h->dev.nodes;                                                                                \
+        view->prim_ids = h->dev.prim_ids;                                                                          \
+        view->tris = h->dev.tris;                                                                                  \
+        view->node_count = h->dev.node_slots - 1;                                                                  \
+        view->prim_count = h->dev.prim_count;                                                                      \
+        view->depth = h->dev.depth;                                                                                \
+        return 0;                                                                                                  \
     }
 
 BVH_IMPL_3D(float, 3f, bvh_intersect_callbackf)

@@ -43,53 +43,6 @@ namespace {
 constexpr int kTraceBlock = 128;
 constexpr int kChunkRays = 128;          // rays claimed per global atomic by one warp
 
-// Shared-memory stack: entry k of thread t lives at base[k * stride + t] (bank = t mod 32).  The stack pointer is kept
-// as ONE 32-bit shared-memory address (a push / pop is a store / load plus one add — indexing base[sp * stride] made the
-// compiler re-derive the thread's base address from S2R in every push and pop of the inner loop), and entry 0 holds a
-// sentinel no node index can equal (all ones: a leaf of 15 primitives at the last representable position), so that
-// try_pop() needs no comparison with the bottom address either.  Callers size the array as depth + 2 entries.
-template <typename U> struct SmemStack {
-    uint32_t top;                                            // shared-window address of the next free entry
-    uint32_t step;                                           // bytes between entries
-    U* base;
-    static constexpr U kSentinel = kTraversalDone<U>;
-    __device__ __forceinline__ SmemStack(U* base_, uint32_t stride, uint32_t) : step(stride * (uint32_t)sizeof(U)), base(base_) {
-        clear();
-        top -= step;
-        push(kSentinel);                                     // (through the same volatile asm as every other access)
-    }
-    __device__ __forceinline__ void clear() { top = (uint32_t)__cvta_generic_to_shared(base) + step; }
-    __device__ __forceinline__ void push(U v) {
-        // (volatile keeps the stack's own loads and stores in program order; no "memory" clobber: nothing else aliases the stack)
-#ifdef BVH_STACK_CLOBBER             // A/B measurements only
-        if constexpr (sizeof(U) == 4) asm volatile("st.shared.b32 [%0], %1;" :: "r"(top), "r"((uint32_t)v) : "memory");
-        else asm volatile("st.shared.b64 [%0], %1;" :: "r"(top), "l"((unsigned long long)v) : "memory");
-#else
-        if constexpr (sizeof(U) == 4) asm volatile("st.shared.b32 [%0], %1;" :: "r"(top), "r"((uint32_t)v));
-        else asm volatile("st.shared.b64 [%0], %1;" :: "r"(top), "l"((unsigned long long)v));
-#endif
-        top += step;
-    }
-    __device__ __forceinline__ U pop() {
-        top -= step;
-#ifdef BVH_STACK_CLOBBER
-        if constexpr (sizeof(U) == 4) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(top) : "memory"); return (U)v; }
-        else { unsigned long long v; asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(top) : "memory"); return (U)v; }
-#else
-        if constexpr (sizeof(U) == 4) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(top)); return (U)v; }
-        else { unsigned long long v; asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(top)); return (U)v; }
-#endif
-    }
-    // pops into `out`; false (and the stack stays empty) when there was nothing to pop
-    __device__ __forceinline__ bool try_pop(U& out) {
-        const U v = pop();
-        if (v == kSentinel) { top += step; return false; }
-        out = v;
-        return true;
-    }
-    __device__ __forceinline__ bool empty() const { return top == (uint32_t)__cvta_generic_to_shared(base) + step; }
-};
-
 __device__ __forceinline__ void load_ray(const DevRay<float>* __restrict__ rays, size_t i, RayCtx<float>& r) {
     const float4* q = reinterpret_cast<const float4*>(rays + i);
     const float4 a = __ldcs(q), b = __ldcs(q + 1);           // streamed once: evict-first

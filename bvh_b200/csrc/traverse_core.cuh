@@ -6,9 +6,10 @@
 // convention is the one every reference caller uses (benchmark.cpp:281-292): test each primitive of
 // the leaf in order and shrink tmax on a hit.
 //
-// The same code runs in three places: the one-thread-per-ray kernel, the persistent kernel (which
-// splits it into an inner phase and a leaf phase, traverse.cu) and the host emulation compiled by
-// g++ for the CPU tests (tests/host_emul.cpp).
+// The same code runs in four places: the one-thread-per-ray kernel, the persistent kernel (which
+// splits it into an inner phase and a leaf phase, traverse.cu), the host emulation compiled by
+// g++ for the CPU tests (tests/host_emul.cpp) and, through traverse_top_down with the caller's leaf,
+// the device traversal API (include/bvh/v2/cuda/intersect.cuh).
 #pragma once
 
 #include "core.cuh"
@@ -163,7 +164,7 @@ template <typename T> inline void load_tri(const DevTri<T>* p, DevTri<T>& o) { o
 template <typename U> constexpr U kTraversalDone = (U)~(U)0;
 
 // The next entry of the stack, or kTraversalDone when it is empty.  The device stack keeps kTraversalDone in its bottom
-// entry (SmemStack, traverse.cu), so there the result is the loaded value itself (the compare only keeps the stack
+// entry (SmemStack, below), so there the result is the loaded value itself (the compare only keeps the stack
 // pointer at the bottom).
 template <typename U, typename Stack> BVH_HD U pop_or_done(Stack& stack) {
     U v = kTraversalDone<U>;
@@ -195,11 +196,10 @@ BVH_HD void inner_step(const DevNode<T>* __restrict__ nodes, const RayCtx<T>& r,
     top = (hit_left || hit_right) ? near_index : pop_or_done<U>(stack);
 }
 
-// Leaf processing (benchmark.cpp:281-292).  stats (nullable): [1] leaves, [2] triangle tests.
+// The triangles [first, first + count) of a leaf (benchmark.cpp:281-292).  stats (nullable): [1] leaves, [2] triangle tests.
 template <typename T>
-BVH_HD void leaf_step(const DevTri<T>* __restrict__ tris, const uint32_t* __restrict__ prim_ids, bool lowest_id,
-                      typename Real<T>::UInt top, RayCtx<T>& r, HitState<T>& hit, uint32_t* stats) {
-    const uint32_t first = (uint32_t)index_first(top), count = index_count(top);
+BVH_HD void leaf_range(const DevTri<T>* __restrict__ tris, const uint32_t* __restrict__ prim_ids, bool lowest_id,
+                       uint32_t first, uint32_t count, RayCtx<T>& r, HitState<T>& hit, uint32_t* stats) {
     if (stats) { stats[1] += 1; stats[2] += count; }
     for (uint32_t i = first; i < first + count; ++i) {
         DevTri<T> tri;
@@ -208,25 +208,131 @@ BVH_HD void leaf_step(const DevTri<T>* __restrict__ tris, const uint32_t* __rest
     }
 }
 
-// Whole traversal for one ray.  stats (nullable): {inner steps, leaves, triangle tests}, the same
+// Leaf processing for the leaf index `top`.
+template <typename T>
+BVH_HD void leaf_step(const DevTri<T>* __restrict__ tris, const uint32_t* __restrict__ prim_ids, bool lowest_id,
+                      typename Real<T>::UInt top, RayCtx<T>& r, HitState<T>& hit, uint32_t* stats) {
+    leaf_range<T>(tris, prim_ids, lowest_id, (uint32_t)index_first(top), index_count(top), r, hit, stats);
+}
+
+// The reference's Bvh::traverse_top_down with the box test of Bvh::intersect (bvh.h:124-182), generic in the leaf and the
+// stack, for one ray whose prologue has been run.  The traversal starts at the node index `start` (a node's packed index:
+// first id << 4 | primitive count) with an empty stack.
+//   leaf_fn(begin, end) -> bool   called on every leaf reached, with its BVH-order primitive range, in the reference's
+//                                 order.  It may shrink r.tmax (or change r.tmin); the next box test reads them.  With kAny
+//                                 a true return ends the traversal.
+//   inner_fn(first_child)         called once per inner step, before the step's box tests, with the reference index of the
+//                                 left child of the inner node being expanded (the right child is first_child + 1).
+//   stack                         push(U) and try_pop(U&) (false when empty); it holds at most depth + 1 entries.
+// A ray whose interval is a NaN misses every box in the reference (each comparison with tmin / tmax fails, node.h:110-115),
+// but traverse_top_down tests no box before its first pop: a leaf `start` is still handed to leaf_fn, and an inner one
+// costs one inner step that finds both children missed.  The device's min / max accumulation does not keep a NaN
+// accumulator (core.cuh acc_max), so such rays go through the branch below, which draws the stacked entries without box
+// tests, exactly what the reference does with them.  The interval is checked again after every leaf call.
+template <typename T, bool kAny, bool kRobust, typename Stack, typename LeafFn, typename InnerFn>
+BVH_HD void traverse_top_down(const DevNode<T>* __restrict__ nodes, RayCtx<T>& r, typename Real<T>::UInt start,
+                              Stack& stack, LeafFn&& leaf_fn, InnerFn&& inner_fn) {
+    using U = typename Real<T>::UInt;
+    U top = start;
+    for (;;) {
+        if (!ray_interval_is_nan(r)) {
+            while (index_count(top) == 0) {
+                inner_fn(index_first(top));
+                inner_step<T, kAny, kRobust>(nodes, r, top, stack);
+            }
+        } else {
+            while (index_count(top) == 0) {
+                inner_fn(index_first(top));
+                top = pop_or_done<U>(stack);                    // both children missed
+            }
+        }
+        if (top == kTraversalDone<U>) break;
+        const U first = index_first(top);
+        const bool was_hit = leaf_fn(first, first + (U)index_count(top));
+        if (kAny && was_hit) break;                             // bvh.h:153-155
+        top = pop_or_done<U>(stack);
+    }
+}
+
+// Whole traversal for one ray with the triangle leaf.  stats (nullable): {inner steps, leaves, triangle tests}, the same
 // three counters the reference exposes through its InnerFn hook (bvh.h:168, benchmark.cpp:282-296).
 template <typename T, bool kAny, bool kRobust, typename Stack>
 BVH_HD void traverse_ray(const DevNode<T>* __restrict__ nodes, const DevTri<T>* __restrict__ tris,
                          const uint32_t* __restrict__ prim_ids, bool lowest_id, typename Real<T>::UInt root_index,
                          RayCtx<T>& r, HitState<T>& hit, Stack& stack, uint32_t* stats) {
     using U = typename Real<T>::UInt;
-    if (ray_interval_is_nan(r)) return;                         // can never hit (node.h:110-115, tri.h:69)
-    U top = root_index;                                         // get_root().index, bvh.h:54
-    for (;;) {
-        while (index_count(top) == 0) {
-            if (stats) stats[0] += 1;
-            inner_step<T, kAny, kRobust>(nodes, r, top, stack);
-        }
-        if (top == kTraversalDone<U>) break;
-        leaf_step<T>(tris, prim_ids, lowest_id, top, r, hit, stats);
-        if (kAny && hit.slot != kInvalidId) break;              // bvh.h:153-155
-        top = pop_or_done<U>(stack);
-    }
+    if (ray_interval_is_nan(r)) return;                         // no triangle can be hit (tri.h:69); counters stay 0
+    traverse_top_down<T, kAny, kRobust>(
+        nodes, r, root_index, stack,                            // get_root().index, bvh.h:54
+        [&](U begin, U end) {
+            leaf_range<T>(tris, prim_ids, lowest_id, (uint32_t)begin, (uint32_t)(end - begin), r, hit, stats);
+            return hit.slot != kInvalidId;
+        },
+        [&](U) { if (stats) stats[0] += 1; });
 }
+
+// A per-thread stack of `Capacity` entries in registers / local memory (the reference's SmallStack, stack.h).  It holds
+// at most depth + 1 entries during a traversal; nothing checks the capacity on the device.
+template <typename U, unsigned Capacity> struct ArrayStack {
+    static constexpr unsigned capacity = Capacity;
+    U elems[Capacity];
+    unsigned size = 0;
+    BVH_HD void push(U v) { elems[size++] = v; }
+    BVH_HD bool try_pop(U& out) {
+        if (size == 0) return false;
+        out = elems[--size];
+        return true;
+    }
+    BVH_HD bool empty() const { return size == 0; }
+};
+
+#if defined(__CUDACC__)
+// Shared-memory stack: entry k of thread t lives at base[k * stride + t] (bank = t mod 32).  The stack pointer is kept
+// as ONE 32-bit shared-memory address (a push / pop is a store / load plus one add — indexing base[sp * stride] made the
+// compiler re-derive the thread's base address from S2R in every push and pop of the inner loop), and entry 0 holds a
+// sentinel no node index can equal (all ones: a leaf of 15 primitives at the last representable position), so that
+// try_pop() needs no comparison with the bottom address either.  Callers size the array as depth + 2 entries.
+template <typename U> struct SmemStack {
+    uint32_t top;                                            // shared-window address of the next free entry
+    uint32_t step;                                           // bytes between entries
+    U* base;
+    static constexpr U kSentinel = kTraversalDone<U>;
+    __device__ __forceinline__ SmemStack(U* base_, uint32_t stride, uint32_t) : step(stride * (uint32_t)sizeof(U)), base(base_) {
+        clear();
+        top -= step;
+        push(kSentinel);                                     // (through the same volatile asm as every other access)
+    }
+    __device__ __forceinline__ void clear() { top = (uint32_t)__cvta_generic_to_shared(base) + step; }
+    __device__ __forceinline__ void push(U v) {
+        // (volatile keeps the stack's own loads and stores in program order; no "memory" clobber: nothing else aliases the stack)
+#ifdef BVH_STACK_CLOBBER             // A/B measurements only
+        if constexpr (sizeof(U) == 4) asm volatile("st.shared.b32 [%0], %1;" :: "r"(top), "r"((uint32_t)v) : "memory");
+        else asm volatile("st.shared.b64 [%0], %1;" :: "r"(top), "l"((unsigned long long)v) : "memory");
+#else
+        if constexpr (sizeof(U) == 4) asm volatile("st.shared.b32 [%0], %1;" :: "r"(top), "r"((uint32_t)v));
+        else asm volatile("st.shared.b64 [%0], %1;" :: "r"(top), "l"((unsigned long long)v));
+#endif
+        top += step;
+    }
+    __device__ __forceinline__ U pop() {
+        top -= step;
+#ifdef BVH_STACK_CLOBBER
+        if constexpr (sizeof(U) == 4) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(top) : "memory"); return (U)v; }
+        else { unsigned long long v; asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(top) : "memory"); return (U)v; }
+#else
+        if constexpr (sizeof(U) == 4) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(top)); return (U)v; }
+        else { unsigned long long v; asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(top)); return (U)v; }
+#endif
+    }
+    // pops into `out`; false (and the stack stays empty) when there was nothing to pop
+    __device__ __forceinline__ bool try_pop(U& out) {
+        const U v = pop();
+        if (v == kSentinel) { top += step; return false; }
+        out = v;
+        return true;
+    }
+    __device__ __forceinline__ bool empty() const { return top == (uint32_t)__cvta_generic_to_shared(base) + step; }
+};
+#endif
 
 } // namespace bvhb200

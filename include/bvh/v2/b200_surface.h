@@ -47,6 +47,7 @@
 #include <vector>
 
 #include <bvh_b200.h>
+#include <bvh_b200_device.h>
 
 #if defined(__GNUC__) || defined(__clang__)
 #define BVH_ALWAYS_INLINE __attribute__((always_inline)) inline
@@ -722,7 +723,8 @@ namespace detail {
 template <typename T> struct CApi;
 template <> struct CApi<float> {
     using Handle = bvh3f; using BBoxPod = bvh_bbox3f; using VecPod = bvh_vec3f; using NodePod = bvh_node3f;
-    using RayPod = bvh_ray3f; using HitPod = bvh_hit3f;
+    using RayPod = bvh_ray3f; using HitPod = bvh_hit3f; using ViewPod = bvh_device_view3f;
+    static int device_view(Handle* h, ViewPod* v) { return bvh3f_get_device_view(h, v); }
     static Handle* build(const BBoxPod* b, const VecPod* c, size_t n, const bvh_build_config* cfg) { return bvh3f_build(nullptr, b, c, n, cfg); }
     static Handle* build_triangles(const float* v, size_t n, const bvh_build_config* cfg, unsigned fl) { return bvh3f_build_triangles(v, n, cfg, fl); }
     static void destroy(Handle* h) { bvh3f_destroy(h); }
@@ -734,7 +736,8 @@ template <> struct CApi<float> {
 };
 template <> struct CApi<double> {
     using Handle = bvh3d; using BBoxPod = bvh_bbox3d; using VecPod = bvh_vec3d; using NodePod = bvh_node3d;
-    using RayPod = bvh_ray3d; using HitPod = bvh_hit3d;
+    using RayPod = bvh_ray3d; using HitPod = bvh_hit3d; using ViewPod = bvh_device_view3d;
+    static int device_view(Handle* h, ViewPod* v) { return bvh3d_get_device_view(h, v); }
     static Handle* build(const BBoxPod* b, const VecPod* c, size_t n, const bvh_build_config* cfg) { return bvh3d_build(nullptr, b, c, n, cfg); }
     static Handle* build_triangles(const double* v, size_t n, const bvh_build_config* cfg, unsigned fl) { return bvh3d_build_triangles(v, n, cfg, fl); }
     static void destroy(Handle* h) { bvh3d_destroy(h); }
@@ -838,6 +841,25 @@ public:
             throw std::runtime_error(std::string("bvh::v2::cuda::Accel::intersect: ") + bvh_last_error());
     }
     typename Api::Handle* handle() const { return handle_; }
+
+    using DeviceViewPod = typename Api::ViewPod;
+    /// The device tree for kernels of your own (bvhNN_get_device_view; in device code wrap it with
+    /// bvh::v2::cuda::DeviceView<T>::from, include/bvh/v2/cuda/intersect.cuh).
+    DeviceViewPod device_view() const {
+        DeviceViewPod v {};
+        if (Api::device_view(handle_, &v))
+            throw std::runtime_error(std::string("bvh::v2::cuda::Accel::device_view: ") + bvh_last_error());
+        return v;
+    }
+    /// Same, for kernels whose per-thread traversal stack holds `stack_capacity` entries: throws std::length_error
+    /// when the tree needs more (depth + 1).  The device never checks a stack's capacity.
+    DeviceViewPod device_view(size_t stack_capacity) const {
+        const DeviceViewPod v = device_view();
+        if (stack_capacity < v.depth + 1)
+            throw std::length_error("bvh::v2::cuda::Accel::device_view: a stack of " + std::to_string(stack_capacity) +
+                                    " entries is too small for a tree of depth " + std::to_string(v.depth));
+        return v;
+    }
 
 private:
     void reset() { if (handle_) Api::destroy(handle_); handle_ = nullptr; }

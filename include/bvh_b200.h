@@ -147,6 +147,9 @@ BVH_API int bvh_optimize_nodes(void* nodes, size_t node_count, int dim, int is_d
 BVH_B200_DECLARE(float, 3f)
 BVH_B200_DECLARE(double, 3d)
 
+/* The device-resident tree of a handle, for CUDA kernels of the caller's own (bvhNN_get_device_view), is declared in
+ * <bvh_b200_device.h>. */
+
 #ifdef __cplusplus
 }
 #endif
