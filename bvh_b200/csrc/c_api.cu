@@ -13,6 +13,7 @@
 #include <bvh_b200_device.h>
 
 #include <algorithm>
+#include <cctype>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -30,34 +31,47 @@ static thread_local std::string g_error;
 void set_error(const std::string& msg) { g_error = msg; }
 const char* last_error() { return g_error.c_str(); }
 
+// The switches of bvh_set_option.  Each setter clamps its value and stores it, or returns false for a value it rejects.
+// Defaults are the initialisers in Tunables (engine.h).
+struct OptionSetter {
+    const char* name;
+    bool (*set)(Tunables&, long);
+};
+static const OptionSetter kOptions[] = {
+    { "morton_bits", [] (Tunables& t, long v) { t.morton_bits = (int)v; return true; } },
+    { "sah_treelets", [] (Tunables& t, long v) { t.sah_treelets = (int)v; return true; } },
+    { "hierarchy", [] (Tunables& t, long v) { t.hierarchy = (int)v; return true; } },
+    { "e2e_chunks", [] (Tunables& t, long v) { t.e2e_chunks = (int)v; return true; } },
+    { "variant", [] (Tunables& t, long v) { if (v != 0 && v != 1) return false; t.variant = (int)v; return true; } },
+    { "use_wide", [] (Tunables& t, long v) { t.use_wide = (int)v; return true; } },
+    { "chunk_rays", [] (Tunables& t, long v) { t.chunk_rays = v < 32 ? 32u : (uint32_t)v; return true; } },
+    { "stack_round", [] (Tunables& t, long v) { t.stack_round = v < 1 ? 1 : (int)v; return true; } },
+    { "smem_carveout", [] (Tunables& t, long v) { t.smem_carveout = (int)v; return true; } },
+    { "refill_min", [] (Tunables& t, long v) { t.refill_min = v < 1 ? 0u : v > 32 ? 32u : (uint32_t)v; return true; } },   // 0: auto
+    { "inner_budget", [] (Tunables& t, long v) { t.inner_budget = v <= 0 ? 0xFFFFFFFFu : (uint32_t)v; return true; } },
+    { "wide_budget", [] (Tunables& t, long v) { t.wide_budget = v <= 0 ? 0xFFFFFFFFu : (uint32_t)v; return true; } },
+    { "watchdog", [] (Tunables& t, long v) { t.watchdog = (uint32_t)v; return true; } },
+    { "gather_staging", [] (Tunables& t, long v) { t.gather_staging = (int)v; return true; } },
+    { "sort_onesweep", [] (Tunables& t, long v) { t.sort_onesweep = (int)v; return true; } },
+    { "treelet_blocks", [] (Tunables& t, long v) { t.treelet_blocks = (int)v; return true; } },
+};
+
+// Initial values: BVH_B200_<NAME> through the same setters (a rejected value keeps the default; unset keeps the default,
+// which for inner_budget is auto).  hierarchy is spelt global / thread64 / thread256 there, anything else is 128.
 Tunables& tunables() {
     static Tunables t;
     static std::once_flag once;
     std::call_once(once, [] {
-        auto env = [] (const char* name, long fallback) { const char* e = getenv(name); return e ? atol(e) : fallback; };
-        t.morton_bits = (int)env("BVH_B200_MORTON_BITS", 0);
-        t.sah_treelets = (int)env("BVH_B200_SAH_TREELETS", -1);
-        if (const char* e = getenv("BVH_B200_HIERARCHY")) {
+        for (const OptionSetter& o : kOptions) {
+            std::string var = "BVH_B200_";
+            for (const char* c = o.name; *c; ++c) var += (char)toupper((unsigned char)*c);
+            const char* e = getenv(var.c_str());
+            if (!e) continue;
             const std::string v = e;
-            t.hierarchy = v == "global" ? 0 : v == "thread64" ? 64 : v == "thread256" ? 256 : 128;
+            const long value = std::string(o.name) != "hierarchy" ? atol(e)
+                             : v == "global" ? 0 : v == "thread64" ? 64 : v == "thread256" ? 256 : 128;
+            o.set(t, value);
         }
-        t.e2e_chunks = (int)env("BVH_B200_E2E_CHUNKS", 0);
-        t.variant = (int)env("BVH_B200_VARIANT", 0);
-        t.use_wide = (int)env("BVH_B200_USE_WIDE", 0);
-        { const long m = env("BVH_B200_REFILL_MIN", 0); t.refill_min = m < 1 ? 0u : m > 32 ? 32u : (uint32_t)m; }   // 0: auto
-        if (getenv("BVH_B200_INNER_BUDGET")) {                  // unset: auto
-            const long budget = env("BVH_B200_INNER_BUDGET", 0);
-            t.inner_budget = budget <= 0 ? 0xFFFFFFFFu : (uint32_t)budget;
-        }
-        const long wbudget = env("BVH_B200_WIDE_BUDGET", 4);
-        t.wide_budget = wbudget <= 0 ? 0xFFFFFFFFu : (uint32_t)wbudget;
-        t.watchdog = (uint32_t)env("BVH_B200_WATCHDOG", 1l << 26);
-        t.stack_round = (int)env("BVH_B200_STACK_ROUND", 2);
-        t.chunk_rays = (uint32_t)env("BVH_B200_CHUNK_RAYS", 64);
-        t.smem_carveout = (int)env("BVH_B200_SMEM_CARVEOUT", -1);
-        t.gather_staging = (int)env("BVH_B200_GATHER_STAGING", 1);
-        t.sort_onesweep = (int)env("BVH_B200_SORT_ONESWEEP", 1);
-        t.treelet_blocks = (int)env("BVH_B200_TREELET_BLOCKS", 3);
     });
     return t;
 }
@@ -670,26 +684,15 @@ BVH_EXPORT void* bvh_host_alloc(size_t bytes) {
 BVH_EXPORT void bvh_host_free(void* ptr) { if (ptr) cudaFreeHost(ptr); }
 BVH_EXPORT int bvh_set_option(const char* name, long value) {
     if (!name) { set_error("set_option: null name"); return -1; }
-    Tunables& t = tunables();
     const std::string n = name;
-    if (n == "morton_bits") t.morton_bits = (int)value;
-    else if (n == "sah_treelets") t.sah_treelets = (int)value;
-    else if (n == "hierarchy") t.hierarchy = (int)value;
-    else if (n == "e2e_chunks") t.e2e_chunks = (int)value;
-    else if (n == "variant") t.variant = (int)value;
-    else if (n == "use_wide") t.use_wide = (int)value;
-    else if (n == "chunk_rays") t.chunk_rays = value < 32 ? 32u : (uint32_t)value;
-    else if (n == "stack_round") t.stack_round = value < 1 ? 1 : (int)value;
-    else if (n == "smem_carveout") t.smem_carveout = (int)value;
-    else if (n == "refill_min") t.refill_min = value < 1 ? 0u : value > 32 ? 32u : (uint32_t)value;     // 0: auto
-    else if (n == "inner_budget") t.inner_budget = value <= 0 ? 0xFFFFFFFFu : (uint32_t)value;
-    else if (n == "wide_budget") t.wide_budget = value <= 0 ? 0xFFFFFFFFu : (uint32_t)value;
-    else if (n == "watchdog") t.watchdog = (uint32_t)value;
-    else if (n == "gather_staging") t.gather_staging = (int)value;
-    else if (n == "sort_onesweep") t.sort_onesweep = (int)value;
-    else if (n == "treelet_blocks") t.treelet_blocks = (int)value;
-    else { set_error("set_option: unknown option " + n); return -1; }
-    return 0;
+    for (const OptionSetter& o : kOptions) {
+        if (n != o.name) continue;
+        if (o.set(tunables(), value)) return 0;
+        set_error("set_option: " + n + " does not accept " + std::to_string(value));
+        return -1;
+    }
+    set_error("set_option: unknown option " + n);
+    return -1;
 }
 BVH_EXPORT int bvh_cuda_trim(int device) {
     if (device < 0 || device >= 64) { set_error("no such CUDA device"); return -1; }

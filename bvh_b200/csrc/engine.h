@@ -9,6 +9,7 @@
 #include <string>
 
 #include "core.cuh"
+#include "trace_plan.h"
 
 namespace bvhb200 {
 
@@ -35,8 +36,8 @@ void device_free(void* ptr, cudaStream_t stream);
 int prepare_device(int device);
 
 // Process-wide switches for experiments and tests; the defaults are the tuned values.  Initialised once from
-// the BVH_B200_* environment variables (DESIGN.md), changed at run time with bvh_set_option — nothing on a
-// call path reads the environment.
+// the BVH_B200_* environment variables (DESIGN.md), changed at run time with bvh_set_option, both through the
+// setters of c_api.cu (kOptions) — nothing on a call path reads the environment.
 struct Tunables {
     std::atomic<int> morton_bits { 0 };         // 0: auto (63 from 2^22 primitives), 30, 63
     std::atomic<int> sah_treelets { -1 };       // -1: by quality (Medium / High), 0 / 1: forced off / on
@@ -44,7 +45,7 @@ struct Tunables {
     std::atomic<int> e2e_chunks { 0 };          // chunks of the host-buffer pipeline, 0: auto
     std::atomic<int> variant { 0 };             // persistent kernel: 0 streaming ray loads, 1 ray chunks staged by bulk async copies (TMA)
     std::atomic<int> use_wide { 0 };            // 1: derive the compressed wide tree with the build and trace with it where its semantics allow
-    std::atomic<uint32_t> inner_budget { 0 };   // inner steps per lane per round, 0: auto (by query kind and kernel, see trace_rays)
+    std::atomic<uint32_t> inner_budget { 0 };   // inner steps per lane per round, 0: auto (by query kind and kernel, see plan_trace)
     std::atomic<uint32_t> refill_min { 0 };     // persistent kernels: idle lanes a warp waits for before it draws new rays (1: at once), 0: auto
     std::atomic<uint32_t> wide_budget { 4 };    // same for the wide kernel
     std::atomic<uint32_t> watchdog { 1u << 26 };
@@ -91,8 +92,6 @@ template <typename T> struct DeviceBvh {
     mutable int last_kernel = 0;        // TraceKernel of the most recent trace_rays call
 };
 
-enum TraceKernel : int { kKernelNone = 0, kKernelPersistentTma, kKernelPersistent, kKernelSimple, kKernelStats, kKernelPair, kKernelWide };
-
 // (Re)derives the wide tree from the binary one, e.g. after an upload from the host mirror.
 // force = false: only if the tree already has one (refresh) or the environment asks for it at build time;
 // force = true: always (first use by a trace).
@@ -124,18 +123,6 @@ template <typename T>
 int export_reference_arrays(const DeviceBvh<T>& bvh, void* d_nodes_out, unsigned long long* d_ids_out, cudaStream_t stream);
 
 template <typename T> void release(DeviceBvh<T>& bvh, cudaStream_t stream);
-
-enum TraceFlags : unsigned {
-    kTraceAnyHit      = 1u << 0,
-    kTraceRobust      = 1u << 1,
-    kTraceLastVisited = 1u << 2,   // reference example tie semantics instead of the canonical lowest id
-    kTraceSimple      = 1u << 8,   // one-thread-per-ray kernel instead of the persistent one
-    kTraceNoTma       = 1u << 9,   // persistent one-lane-per-ray kernel, rays read with streaming loads
-    kTraceTma         = 1u << 10,  // persistent one-lane-per-ray kernel, ray chunks staged by bulk async copy (TMA)
-    kTracePair        = 1u << 11,  // persistent lane-pair kernel (two lanes per ray)
-    kTraceWide        = 1u << 12,  // persistent kernel over the compressed 4-wide tree
-    kTraceSortRays    = 1u << 13,  // traverse the batch in the Morton order of the ray origins (results stay in the caller's order)
-};
 
 // Fused multi-GPU gather: besides (or instead of) the local hit array, every finished ray's record is
 // stored at element `offset + i` of the gathered hit array of each rank — peer[] holds that array's address

@@ -41,17 +41,23 @@ namespace {
 #define BVH_TRACE_BLOCKS 9
 #endif
 constexpr int kTraceBlock = 128;
-constexpr int kChunkRays = 128;          // rays claimed per global atomic by one warp
+constexpr uint32_t kPairRunRays = 128;   // the lane-pair kernel's runs: fixed, the chunk_rays switch does not apply to it
 
-__device__ __forceinline__ void load_ray(const DevRay<float>* __restrict__ rays, size_t i, RayCtx<float>& r) {
-    const float4* q = reinterpret_cast<const float4*>(rays + i);
-    const float4 a = __ldcs(q), b = __ldcs(q + 1);           // streamed once: evict-first
+// One ray record into registers.  kStreamed: from global memory, read once (ld.global.cs, evict-first); otherwise a plain
+// load (the TMA kernel's shared-memory copy of the rays).
+template <bool kStreamed, typename V> __device__ __forceinline__ V load_ray_piece(const V* p) { return kStreamed ? __ldcs(p) : *p; }
+template <bool kStreamed = true>
+__device__ __forceinline__ void load_ray(const DevRay<float>* p, RayCtx<float>& r) {
+    const float4* q = reinterpret_cast<const float4*>(p);
+    const float4 a = load_ray_piece<kStreamed>(q), b = load_ray_piece<kStreamed>(q + 1);
     r.org[0] = a.x; r.org[1] = a.y; r.org[2] = a.z; r.dir[0] = a.w;
     r.dir[1] = b.x; r.dir[2] = b.y; r.tmin = b.z; r.tmax = b.w;
 }
-__device__ __forceinline__ void load_ray(const DevRay<double>* __restrict__ rays, size_t i, RayCtx<double>& r) {
-    const double2* q = reinterpret_cast<const double2*>(rays + i);
-    const double2 a = __ldcs(q), b = __ldcs(q + 1), c = __ldcs(q + 2), d = __ldcs(q + 3);
+template <bool kStreamed = true>
+__device__ __forceinline__ void load_ray(const DevRay<double>* p, RayCtx<double>& r) {
+    const double2* q = reinterpret_cast<const double2*>(p);
+    const double2 a = load_ray_piece<kStreamed>(q), b = load_ray_piece<kStreamed>(q + 1);
+    const double2 c = load_ray_piece<kStreamed>(q + 2), d = load_ray_piece<kStreamed>(q + 3);
     r.org[0] = a.x; r.org[1] = a.y; r.org[2] = b.x; r.dir[0] = b.y;
     r.dir[1] = c.x; r.dir[2] = c.y; r.tmin = d.x; r.tmax = d.y;
 }
@@ -73,34 +79,33 @@ __device__ __forceinline__ void multimem_store_v4(void* p, uint4 v) {
 }
 
 // A miss reports id = all ones (BVH_INVALID_PRIM_ID), t = the ray's tmax, u = v = 0.
-__device__ __forceinline__ void store_hit(const HitSinks<float>& sinks, size_t i, const HitState<float>& h,
-                                          float tmax, const uint32_t* __restrict__ prim_ids) {
-    uint4 o;
+template <typename T>
+__device__ __forceinline__ DevHit<T> make_record(const HitState<T>& h, T tmax, const uint32_t* __restrict__ prim_ids) {
+    DevHit<T> rec;
     const bool was_hit = h.slot != kInvalidId;
-    o.x = was_hit ? prim_ids[h.slot] : kInvalidId;
-    o.y = __float_as_uint(was_hit ? h.t : tmax);
-    o.z = __float_as_uint(was_hit ? h.u : 0.f);
-    o.w = __float_as_uint(was_hit ? h.v : 0.f);
-    if (sinks.local) __stcs(reinterpret_cast<uint4*>(sinks.local + i), o);
-    if (sinks.multicast) multimem_store_v4(sinks.multicast + i, o);
-    else for (int p = 0; p < sinks.peer_count; ++p) *reinterpret_cast<uint4*>(sinks.peer[p] + i) = o;
+    rec.prim_id = was_hit ? (decltype(rec.prim_id))prim_ids[h.slot] : (decltype(rec.prim_id))~(decltype(rec.prim_id))0;
+    rec.t = was_hit ? h.t : tmax;
+    rec.u = was_hit ? h.u : (T)0;
+    rec.v = was_hit ? h.v : (T)0;
+    return rec;
 }
-__device__ __forceinline__ void store_hit(const HitSinks<double>& sinks, size_t i, const HitState<double>& h,
-                                          double tmax, const uint32_t* __restrict__ prim_ids) {
-    const bool was_hit = h.slot != kInvalidId;
-    ulonglong2 a, b;
-    a.x = was_hit ? (unsigned long long)prim_ids[h.slot] : ~0ull;
-    a.y = (unsigned long long)__double_as_longlong(was_hit ? h.t : tmax);
-    b.x = (unsigned long long)__double_as_longlong(was_hit ? h.u : 0.0);
-    b.y = (unsigned long long)__double_as_longlong(was_hit ? h.v : 0.0);
+
+// One record to every sink with one store per sink (16-byte pieces).
+template <typename T>
+__device__ __forceinline__ void store_record_direct(const HitSinks<T>& sinks, unsigned long long i, const DevHit<T>& rec) {
+    using V = typename std::conditional<sizeof(T) == 4, uint4, ulonglong2>::type;
+    constexpr int kParts = (int)(sizeof(DevHit<T>) / 16);
+    const V* src = reinterpret_cast<const V*>(&rec);
     if (sinks.local) {
-        ulonglong2* d = reinterpret_cast<ulonglong2*>(sinks.local + i);
-        __stcs(d, a);
-        __stcs(d + 1, b);
+        V* d = reinterpret_cast<V*>(sinks.local + i);
+        #pragma unroll
+        for (int k = 0; k < kParts; ++k) __stcs(d + k, src[k]);
     }
+    if (sizeof(T) == 4 && sinks.multicast) { multimem_store_v4(sinks.multicast + i, *reinterpret_cast<const uint4*>(&rec)); return; }
     for (int p = 0; p < sinks.peer_count; ++p) {
-        ulonglong2* d = reinterpret_cast<ulonglong2*>(sinks.peer[p] + i);
-        d[0] = a; d[1] = b;
+        V* d = reinterpret_cast<V*>(sinks.peer[p] + i);
+        #pragma unroll
+        for (int k = 0; k < kParts; ++k) d[k] = src[k];
     }
 }
 
@@ -116,9 +121,7 @@ template <typename T> struct TraceArgs {
     uint32_t stack_entries;
     const WideNode* wide;             // compressed 4-wide tree (float only) or nullptr
     uint32_t wide_entries;            // stack entries per thread for the wide kernel
-    int variant;                      // 0/1: one lane per ray (direct / TMA-staged rays), 2: lane-pair kernel
-    bool use_tma;                     // persistent kernel: stage ray chunks with cp.async.bulk
-    uint32_t inner_budget;            // persistent kernel: inner steps per lane per round (0xFFFFFFFF = unbounded)
+    uint32_t inner_budget;           // persistent kernel: inner steps per lane per round (0xFFFFFFFF = unbounded)
     uint32_t chunk_rays;              // persistent kernels: consecutive rays a warp claims with one global atomic (multiple of 32)
     uint32_t refill_min;              // persistent kernels: idle lanes a warp waits for before it draws new rays (1: refill at once)
     uint32_t full_mask;               // 0xFFFFFFFF passed at run time (see trace_pair_kernel)
@@ -138,7 +141,7 @@ trace_simple_kernel(TraceArgs<T> a) {
     if (i >= a.n) return;
     SmemStack<U> stack { reinterpret_cast<U*>(smem_raw) + threadIdx.x, kTraceBlock, 0 };
     RayCtx<T> r;
-    load_ray(a.rays, i, r);
+    load_ray(a.rays + i, r);
     ray_prologue<T, kRobust>(r);
     HitState<T> hit { kInvalidId, r.tmax, (T)0, (T)0 };
     const T tmax_in = r.tmax;
@@ -146,7 +149,7 @@ trace_simple_kernel(TraceArgs<T> a) {
     const U root_index = a.nodes[1].index;
     traverse_ray<T, kAny, kRobust>(a.nodes, a.tris, a.prim_ids, a.lowest_id != 0, root_index, r, hit, stack,
                                    kStats ? stats : nullptr);
-    store_hit(a.hits, i, hit, tmax_in, a.prim_ids);
+    store_record_direct(a.hits, i, make_record(hit, tmax_in, a.prim_ids));
     if (kStats) {
         a.ray_stats[3 * i + 0] = stats[0];
         a.ray_stats[3 * i + 1] = stats[1];
@@ -236,24 +239,6 @@ template <typename T> struct HitStager {
         return (buf && cur < (uint32_t)kStageSlots) ? (cur << 5) | (uint32_t)(ray_index & 31ull) : kNoTag;
     }
 };
-
-template <typename T>
-__device__ __forceinline__ void store_record_direct(const HitSinks<T>& sinks, unsigned long long i, const DevHit<T>& rec) {
-    using V = typename std::conditional<sizeof(T) == 4, uint4, ulonglong2>::type;
-    constexpr int kParts = (int)(sizeof(DevHit<T>) / 16);
-    const V* src = reinterpret_cast<const V*>(&rec);
-    if (sinks.local) {
-        V* d = reinterpret_cast<V*>(sinks.local + i);
-        #pragma unroll
-        for (int k = 0; k < kParts; ++k) __stcs(d + k, src[k]);
-    }
-    if (sizeof(T) == 4 && sinks.multicast) { multimem_store_v4(sinks.multicast + i, *reinterpret_cast<const uint4*>(&rec)); return; }
-    for (int p = 0; p < sinks.peer_count; ++p) {
-        V* d = reinterpret_cast<V*>(sinks.peer[p] + i);
-        #pragma unroll
-        for (int k = 0; k < kParts; ++k) d[k] = src[k];
-    }
-}
 
 // All lanes of the warp call the functions below together (converged code); every lane reads the same shared words,
 // lane 0 writes them back, a __syncwarp() separates the two.
@@ -351,28 +336,100 @@ __device__ __forceinline__ void stager_retire(HitStager<T>& st, const HitSinks<T
     }
 }
 
-template <typename T>
-__device__ __forceinline__ DevHit<T> make_record(const HitState<T>& h, T tmax, const uint32_t* __restrict__ prim_ids) {
-    DevHit<T> rec;
-    const bool was_hit = h.slot != kInvalidId;
-    rec.prim_id = was_hit ? (decltype(rec.prim_id))prim_ids[h.slot] : (decltype(rec.prim_id))~(decltype(rec.prim_id))0;
-    rec.t = was_hit ? h.t : tmax;
-    rec.u = was_hit ? h.u : (T)0;
-    rec.v = was_hit ? h.v : (T)0;
-    return rec;
+// One finished ray: through the warp's staging slots in gather mode, else straight to the sinks.
+template <typename T, bool kGather>
+__device__ __forceinline__ void retire_ray(HitStager<T>& st, const HitSinks<T>& sinks, unsigned long long i, const HitState<T>& h,
+                                           T tmax, const uint32_t* __restrict__ prim_ids) {
+    if (kGather) stager_retire(st, sinks, i, make_record(h, tmax, prim_ids));
+    else store_record_direct(sinks, i, make_record(h, tmax, prim_ids));
 }
 
-__device__ __forceinline__ void read_ray_smem(const DevRay<float>* p, RayCtx<float>& r) {
-    const float4* q = reinterpret_cast<const float4*>(p);
-    const float4 a = q[0], b = q[1];
-    r.org[0] = a.x; r.org[1] = a.y; r.org[2] = a.z; r.dir[0] = a.w;
-    r.dir[1] = b.x; r.dir[2] = b.y; r.tmin = b.z; r.tmax = b.w;
+// ---- the ray feed of the persistent kernels ------------------------------------------------------------------
+// A warp claims private runs of consecutive batch positions with one global atomicAdd per run and hands them to its idle
+// lanes by ballot + prefix rank (active-mask compaction).  A warp draws new rays only once refill_min of its lanes are
+// idle: the rays drawn together are neighbours (consecutive positions of one run) and start at the root in the same
+// iteration, so they stay in step through the top of the tree and their node fetches — same address in the same
+// instruction — cost one L1 wavefront instead of one per lane; the price is idle lanes, which these L1-bound kernels can
+// afford.
+
+// A round past the watchdog's limit sets the status word: a hang becomes an error (see trace_rays).
+__device__ __forceinline__ bool watchdog_fired(uint32_t& rounds, uint32_t limit, uint32_t* status, unsigned lane) {
+    if (++rounds <= limit) return false;
+    if (lane == 0) atomicExch(status, 1u);
+    return true;
 }
-__device__ __forceinline__ void read_ray_smem(const DevRay<double>* p, RayCtx<double>& r) {
-    const double2* q = reinterpret_cast<const double2*>(p);
-    const double2 a = q[0], b = q[1], c = q[2], d = q[3];
-    r.org[0] = a.x; r.org[1] = a.y; r.org[2] = b.x; r.dir[0] = b.y;
-    r.dir[1] = c.x; r.dir[2] = c.y; r.tmin = d.x; r.tmax = d.y;
+
+// First position of a new run of `run` positions (warp-uniform; it may lie beyond the batch).
+__device__ __forceinline__ unsigned long long claim_run(unsigned long long* next_ray, uint32_t run, unsigned lane, unsigned mask) {
+    unsigned long long first = 0;
+    if (lane == 0) first = atomicAdd(next_ray, (unsigned long long)run);
+    return __shfl_sync(mask, first, 0);
+}
+
+// The rest of the warp's current run, and whether the batch has no rays left (warp-uniform).
+struct RunCursor {
+    unsigned long long pos = 0, end = 0;
+    bool exhausted = false;
+};
+
+// One draw: the lanes of `idle` (`rank`: this lane's rank among them) take the next popc(idle) positions of the run at
+// most, clipped to the batch and, in gather mode, to the staging group of 32 consecutive rays the run is in.  Claims a new
+// run when the current one is used up; returns false, with `exhausted` set, when the batch has none left.  `got` is set
+// when this lane drew a ray; its index (through the `order` indirection when there is one) goes to `index`, the ray to `r`.
+template <typename T, bool kGather>
+__device__ __forceinline__ bool draw_from_run(RunCursor& c, const TraceArgs<T>& a, uint32_t run, unsigned idle, unsigned rank,
+                                              bool lane_idle, HitStager<T>& stager, unsigned lane, unsigned mask,
+                                              unsigned long long& index, RayCtx<T>& r, bool& got) {
+    if (c.pos == c.end) {
+        const unsigned long long first = claim_run(a.next_ray, run, lane, mask);
+        if (first >= a.n) { c.exhausted = true; return false; }
+        c.pos = first;
+        c.end = first + run < a.n ? first + run : a.n;
+    }
+    unsigned avail = (unsigned)(c.end - c.pos);
+    const unsigned want = __popc(idle);
+    if (kGather) {                                  // never draw across a staging group's boundary
+        const unsigned in_group = (unsigned)(c.pos & 31ull);
+        if (in_group == 0) stager_open(stager, a.hits, c.pos >> 5, avail < 32u ? avail : 32u, lane);
+        if (avail > 32u - in_group) avail = 32u - in_group;
+    }
+    const unsigned take = want < avail ? want : avail;
+    if (lane_idle && rank < take) {
+        index = c.pos + rank;
+        if (a.order) index = a.order[index];
+        load_ray(a.rays + index, r);
+        got = true;
+    }
+    c.pos += take;
+    return true;
+}
+
+// Starts a ray a lane has just drawn: a miss at its tmax so far and, in gather mode, its staging slot.  A ray whose
+// interval is a NaN can hit nothing: it retires at once as a miss and false is returned.
+template <typename T, bool kGather, typename Retire>
+__device__ __forceinline__ bool start_ray(const RayCtx<T>& r, HitState<T>& hit, T& tmax_in, HitStager<T>& stager,
+                                          unsigned long long index, Retire&& retire) {
+    tmax_in = r.tmax;
+    hit.slot = kInvalidId; hit.t = r.tmax; hit.u = (T)0; hit.v = (T)0;
+    if (kGather) stager.tag = stager.tag_for(index);
+    if (ray_interval_is_nan(r)) { retire(); return false; }
+    return true;
+}
+
+// Refills the warp's idle lanes among `lanes`, once refill_min of them are idle, until none is idle or the batch has no
+// rays left.  draw(idle, rank) hands out one round of rays (rank: the lane's rank in `idle`, counted over lt_mask); it
+// returns false when the batch has none left.
+template <typename T, bool kGather, typename Draw>
+__device__ __forceinline__ void refill_lanes(const bool& has_ray, const RunCursor& c, unsigned lanes, uint32_t refill_min,
+                                             unsigned lt_mask, unsigned mask, HitStager<T>& stager, const HitSinks<T>& sinks,
+                                             unsigned lane, Draw&& draw) {
+    unsigned idle = __ballot_sync(mask, !has_ray) & lanes;
+    if ((uint32_t)__popc(idle) < refill_min) idle = 0u;
+    while (idle != 0u && !c.exhausted) {
+        if (!draw(idle, (unsigned)__popc(idle & lt_mask))) break;
+        if (kGather) stager_account(stager, sinks, lane);      // (a NaN ray may just have been retired)
+        idle = __ballot_sync(mask, !has_ray) & lanes;
+    }
 }
 
 constexpr int kTmaChunkRays = 32;        // rays per bulk copy (1 KB of float rays), two buffers per warp
@@ -398,9 +455,7 @@ trace_persistent_kernel(TraceArgs<T> a) {
     const U root_index = a.nodes[1].index;
     const uint32_t inner_budget = a.inner_budget;
 
-    // warp-uniform cursor over the warp's private chunk(s) of rays
-    unsigned long long chunk_pos = 0, chunk_end = 0;           // !kTma: global ray indices
-    bool exhausted = false;
+    RunCursor run;                  // (kTma: its end is not clipped to the batch; the count of each staged chunk is)
     // kTma state (warp-uniform)
     // (kept as scalars selected by `cur`, not arrays, so that nothing is spilled to local memory)
     DevRay<T>* ray_buf0 = nullptr; DevRay<T>* ray_buf1 = nullptr;
@@ -409,15 +464,12 @@ trace_persistent_kernel(TraceArgs<T> a) {
     uint32_t cur = 0, buf_pos = 0;
 
     auto prefetch = [&] (uint32_t b) {      // stage the next 32 rays of the warp's private run (claiming a new run when it is used up)
-        if (chunk_pos == chunk_end) {
-            unsigned long long first = 0;
-            if (lane == 0) first = atomicAdd(a.next_ray, (unsigned long long)a.chunk_rays);
-            first = __shfl_sync(kFull, first, 0);
-            chunk_pos = first;
-            chunk_end = first + a.chunk_rays;               // (may lie beyond n: the count below is clipped)
+        if (run.pos == run.end) {
+            run.pos = claim_run(a.next_ray, a.chunk_rays, lane, kFull);
+            run.end = run.pos + a.chunk_rays;
         }
-        const unsigned long long base = chunk_pos;
-        chunk_pos += kTmaChunkRays;
+        const unsigned long long base = run.pos;
+        run.pos += kTmaChunkRays;
         uint32_t cnt = 0;
         if (base < a.n) cnt = (uint32_t)(base + kTmaChunkRays < a.n ? kTmaChunkRays : a.n - base);
         if (b == 0) { count0 = cnt; base0 = base; } else { count1 = cnt; base1 = base; }
@@ -435,10 +487,6 @@ trace_persistent_kernel(TraceArgs<T> a) {
         unsigned char* stage_base = smem_raw + (size_t)a.stack_entries * kTraceBlock * sizeof(U) + (kTma ? tma_smem_bytes<T>() : 0);
         stager.init(stage_base, warp, lane, a.stage_hits);
     }
-    auto retire = [&] (unsigned long long index, const HitState<T>& h, T tmax) {
-        if (kGather) stager_retire(stager, a.hits, index, make_record(h, tmax, a.prim_ids));
-        else store_hit(a.hits, index, h, tmax, a.prim_ids);
-    };
 
     if (kTma) {
         unsigned char* tma_base = smem_raw + (size_t)a.stack_entries * kTraceBlock * sizeof(U);
@@ -460,86 +508,49 @@ trace_persistent_kernel(TraceArgs<T> a) {
     HitState<T> hit;
     T tmax_in = (T)0;
     U top = 0;
+    auto retire = [&] { retire_ray<T, kGather>(stager, a.hits, ray_index, hit, tmax_in, a.prim_ids); };
+
+    // one draw: from the staged chunk (kTma) or straight from the run
+    auto draw = [&] (unsigned idle, unsigned rank) {
+        bool got = false;
+        if (kTma) {
+            const uint32_t cur_count = cur == 0 ? count0 : count1;
+            if (cur_count == 0) { run.exhausted = true; return false; }
+            const uint32_t cur_bar = cur == 0 ? bar0 : bar1, cur_phase = cur == 0 ? phase0 : phase1;
+            while (!mbar_try_wait(cur_bar, cur_phase)) { }
+            if (kGather && buf_pos == 0) stager_open(stager, a.hits, (cur == 0 ? base0 : base1) >> 5, cur_count, lane);
+            const unsigned avail = cur_count - buf_pos, want = __popc(idle);
+            const unsigned take = want < avail ? want : avail;
+            if (!has_ray && rank < take) {
+                ray_index = (cur == 0 ? base0 : base1) + buf_pos + rank;
+                load_ray<false>((cur == 0 ? ray_buf0 : ray_buf1) + buf_pos + rank, r);
+                got = true;
+            }
+            buf_pos += take;
+            if (buf_pos == cur_count) {                    // buffer drained: re-arm it with the next chunk
+                __syncwarp();
+                if (cur == 0) phase0 ^= 1u; else phase1 ^= 1u;
+                prefetch(cur);
+                cur ^= 1u; buf_pos = 0;
+            }
+        } else {
+            if (!draw_from_run<T, kGather>(run, a, a.chunk_rays, idle, rank, !has_ray, stager, lane, kFull, ray_index, r, got)) return false;
+        }
+        if (got && start_ray<T, kGather>(r, hit, tmax_in, stager, ray_index, retire)) {
+            ray_prologue<T, kRobust>(r);
+            top = root_index;
+            stack.clear();
+            has_ray = true;
+        }
+        return true;
+    };
 
     uint32_t rounds = 0;
     for (;;) {
-        if (++rounds > a.watchdog) {                       // a hang becomes an error (see trace_rays)
-            if (lane == 0) atomicExch(a.status, 1u);
-            return;
-        }
-        // ---- refill idle lanes from the private chunk (claiming a new chunk when it runs dry) ----
-        // A warp draws new rays only once refill_min of its lanes are idle.  The rays drawn together are neighbours
-        // (consecutive indices of one chunk) and start at the root in the same iteration, so they stay in step through
-        // the top of the tree and their node fetches — same address in the same instruction — cost one L1 wavefront
-        // instead of one per lane; the price is idle lanes, which this L1-bound kernel can afford.
-        unsigned idle = __ballot_sync(kFull, !has_ray);
-        if ((uint32_t)__popc(idle) < a.refill_min) idle = 0u;
-        while (idle != 0u && !exhausted) {
-            unsigned take, rank = __popc(idle & lt_mask);
-            bool got = false;
-            if (kTma) {
-                const uint32_t cur_count = cur == 0 ? count0 : count1;
-                if (cur_count == 0) { exhausted = true; break; }
-                const uint32_t cur_bar = cur == 0 ? bar0 : bar1, cur_phase = cur == 0 ? phase0 : phase1;
-                while (!mbar_try_wait(cur_bar, cur_phase)) { }
-                if (kGather && buf_pos == 0) stager_open(stager, a.hits, (cur == 0 ? base0 : base1) >> 5, cur_count, lane);
-                const unsigned avail = cur_count - buf_pos, want = __popc(idle);
-                take = want < avail ? want : avail;
-                if (!has_ray && rank < take) {
-                    ray_index = (cur == 0 ? base0 : base1) + buf_pos + rank;
-                    read_ray_smem((cur == 0 ? ray_buf0 : ray_buf1) + buf_pos + rank, r);
-                    got = true;
-                }
-                buf_pos += take;
-                if (buf_pos == cur_count) {                // buffer drained: re-arm it with the next chunk
-                    __syncwarp();
-                    if (cur == 0) phase0 ^= 1u; else phase1 ^= 1u;
-                    prefetch(cur);
-                    cur ^= 1u; buf_pos = 0;
-                }
-            } else {
-                if (chunk_pos == chunk_end) {
-                    unsigned long long base = 0;
-                    if (lane == 0) base = atomicAdd(a.next_ray, (unsigned long long)a.chunk_rays);
-                    base = __shfl_sync(kFull, base, 0);
-                    if (base >= a.n) { exhausted = true; break; }
-                    chunk_pos = base;
-                    chunk_end = base + a.chunk_rays < a.n ? base + a.chunk_rays : a.n;
-                }
-                unsigned avail = (unsigned)(chunk_end - chunk_pos);
-                const unsigned want = __popc(idle);
-                if (kGather) {                              // one staging group = 32 consecutive rays: never draw across a boundary
-                    const unsigned in_group = (unsigned)(chunk_pos & 31ull);
-                    if (in_group == 0) stager_open(stager, a.hits, chunk_pos >> 5, avail < 32u ? avail : 32u, lane);
-                    if (avail > 32u - in_group) avail = 32u - in_group;
-                }
-                take = want < avail ? want : avail;
-                if (!has_ray && rank < take) {
-                    ray_index = chunk_pos + rank;
-                    if (a.order) ray_index = a.order[ray_index];
-                    load_ray(a.rays, ray_index, r);
-                    got = true;
-                }
-                chunk_pos += take;
-            }
-            if (got) {
-                tmax_in = r.tmax;
-                hit.slot = kInvalidId; hit.t = r.tmax; hit.u = (T)0; hit.v = (T)0;
-                if (kGather) stager.tag = stager.tag_for(ray_index);
-                if (ray_interval_is_nan(r)) {
-                    retire(ray_index, hit, tmax_in);                             // can never hit: retire as a miss
-                } else {
-                    ray_prologue<T, kRobust>(r);
-                    top = root_index;
-                    stack.clear();
-                    has_ray = true;
-                }
-            }
-            if (kGather) stager_account(stager, a.hits, lane);      // (a NaN ray may just have been retired)
-            idle = __ballot_sync(kFull, !has_ray);
-        }
+        if (watchdog_fired(rounds, a.watchdog, a.status, lane)) return;
+        refill_lanes<T, kGather>(has_ray, run, kFull, a.refill_min, lt_mask, kFull, stager, a.hits, lane, draw);
         if (__ballot_sync(kFull, has_ray) == 0u) {
-            if (exhausted) break;                            // nothing in flight and nothing left
+            if (run.exhausted) break;                        // nothing in flight and nothing left
             continue;                                        // (only NaN rays were drawn: refill again)
         }
 
@@ -552,7 +563,7 @@ trace_persistent_kernel(TraceArgs<T> a) {
                 inner_step<T, kAny, kRobust>(a.nodes, r, top, stack);
             }
             if (top == kTraversalDone<U>) {
-                retire(ray_index, hit, tmax_in);
+                retire();
                 has_ray = false;
             }
         }
@@ -562,7 +573,7 @@ trace_persistent_kernel(TraceArgs<T> a) {
         if (has_ray && index_count(top) != 0) {
             leaf_step<T>(a.tris, a.prim_ids, lowest_id, top, r, hit, nullptr);
             if ((kAny && hit.slot != kInvalidId) || !stack.try_pop(top)) {
-                retire(ray_index, hit, tmax_in);
+                retire();
                 has_ray = false;
             }
         }
@@ -574,10 +585,10 @@ trace_persistent_kernel(TraceArgs<T> a) {
 
 // ---- lane-pair kernel ------------------------------------------------------------------------------
 // Two adjacent lanes serve ONE ray: in an inner step lane 0 of the pair fetches and tests the left
-// child, lane 1 the right child (one 256-bit load each, both from the same 64-byte block), and the two
-// exchange (hit, entry distance, index) with pair-masked __ballot_sync / __shfl_xor_sync.  Why: with
-// divergent rays the L1 data pipe spends one wavefront per thread per load (profiles/: the one-lane-per-ray
-// kernel is bound by l1tex__data_pipe_lsu_wavefronts at ~87 % of peak); the two lanes of a pair hit the same
+// child, lane 1 the right child (each a 32-byte node, two 128-bit loads, both nodes from the same 64-byte block), and
+// the two exchange (hit, entry distance, index) with pair-masked __ballot_sync / __shfl_xor_sync.  Why: with
+// divergent rays the L1 data pipe spends one wavefront per thread per load (the one-lane-per-ray kernel was
+// measured bound by l1tex__data_pipe_lsu_wavefronts at ~87 % of peak on an earlier GPU); the two lanes of a pair hit the same
 // line, so a whole sibling pair costs ONE wavefront instead of two.  Control state (top, stack pointer,
 // tmax, hit) is replicated in both lanes, which take identical decisions; the leaf phase is executed
 // redundantly by both lanes (same addresses, so no extra memory wavefronts).  Per-ray semantics are
@@ -607,8 +618,8 @@ trace_pair_kernel(TraceArgs<T> a) {
     const U root_index = a.nodes[1].index;
     const uint32_t inner_budget = a.inner_budget;
 
-    unsigned long long chunk_pos = 0, chunk_end = 0;                   // warp-uniform
-    bool exhausted = false;
+    RunCursor run;
+    HitStager<T> stager;                                               // (no gather mode: unused)
 
     bool has_ray = false;
     unsigned long long ray_index = 0;
@@ -616,49 +627,32 @@ trace_pair_kernel(TraceArgs<T> a) {
     HitState<T> hit;
     T tmax_in = (T)0;
     U top = 0;
+    // both lanes of a pair hold the ray; the even one stores its record
+    auto retire = [&] { if (sub == 0) store_record_direct(a.hits, ray_index, make_record(hit, tmax_in, a.prim_ids)); };
+
+    // Pairs are drawn like lanes, through the even lanes (the odd lane of a pair has its partner's rank), with no
+    // refill threshold: every idle pair is refilled at once.  (Rays are never sorted for this kernel: `order` is null.)
+    auto draw = [&] (unsigned idle, unsigned rank) {
+        bool got = false;
+        if (!draw_from_run<T, false>(run, a, kPairRunRays, idle, rank, !has_ray, stager, lane, kFull, ray_index, r, got)) return false;
+        if (got && start_ray<T, false>(r, hit, tmax_in, stager, ray_index, retire)) {
+            ray_prologue<T, kRobust>(r);
+            top = root_index;
+            stack.clear();
+            has_ray = true;
+        }
+        return true;
+    };
 
     // `lane_zero` is 0 for every thread (blocks have 128 threads) but not provably so: adding it keeps the
     // round counters in ordinary per-lane registers instead of a warp-uniform register shared by the warp.
     const uint32_t lane_zero = threadIdx.x >> 10;
     uint32_t rounds = lane_zero;
     for (;;) {
-        if (++rounds > a.watchdog) {                       // a hang becomes an error (see trace_rays)
-            if (lane == 0) atomicExch(a.status, 1u);
-            return;
-        }
-        // ---- refill idle pairs -----------------------------------------------------------------------
-        unsigned idle = __ballot_sync(kFull, !has_ray) & kEven;
-        while (idle != 0u && !exhausted) {
-            if (chunk_pos == chunk_end) {
-                unsigned long long base = 0;
-                if (lane == 0) base = atomicAdd(a.next_ray, (unsigned long long)kChunkRays);
-                base = __shfl_sync(kFull, base, 0);
-                if (base >= a.n) { exhausted = true; break; }
-                chunk_pos = base;
-                chunk_end = base + kChunkRays < a.n ? base + kChunkRays : a.n;
-            }
-            const unsigned avail = (unsigned)(chunk_end - chunk_pos), want = __popc(idle);
-            const unsigned take = want < avail ? want : avail;
-            const unsigned rank = __popc(idle & lt_mask);
-            if (!has_ray && rank < take) {
-                ray_index = chunk_pos + rank;
-                load_ray(a.rays, ray_index, r);
-                tmax_in = r.tmax;
-                hit.slot = kInvalidId; hit.t = r.tmax; hit.u = (T)0; hit.v = (T)0;
-                if (ray_interval_is_nan(r)) {
-                    if (sub == 0) store_hit(a.hits, ray_index, hit, tmax_in, a.prim_ids);
-                } else {
-                    ray_prologue<T, kRobust>(r);
-                    top = root_index;
-                    stack.clear();
-                    has_ray = true;
-                }
-            }
-            chunk_pos += take;
-            idle = __ballot_sync(kFull, !has_ray) & kEven;
-        }
+        if (watchdog_fired(rounds, a.watchdog, a.status, lane)) return;
+        refill_lanes<T, false>(has_ray, run, kEven, 0u, lt_mask, kFull, stager, a.hits, lane, draw);
         if (__ballot_sync(kFull, has_ray) == 0u) {
-            if (exhausted) break;
+            if (run.exhausted) break;
             continue;
         }
 
@@ -696,7 +690,7 @@ trace_pair_kernel(TraceArgs<T> a) {
                 if (active) top = next;
                 if (finished) { has_ray = false; retired = true; }
             }
-            if (retired && sub == 0) store_hit(a.hits, ray_index, hit, tmax_in, a.prim_ids);
+            if (retired) retire();
         }
         __syncwarp(kFull);
 
@@ -704,7 +698,7 @@ trace_pair_kernel(TraceArgs<T> a) {
         if (has_ray && index_count(top) != 0) {
             leaf_step<T>(a.tris, a.prim_ids, lowest_id, top, r, hit, nullptr);
             if ((kAny && hit.slot != kInvalidId) || stack.empty()) {
-                if (sub == 0) store_hit(a.hits, ray_index, hit, tmax_in, a.prim_ids);
+                retire();
                 has_ray = false;
             } else {
                 top = stack.pop();
@@ -717,7 +711,7 @@ trace_pair_kernel(TraceArgs<T> a) {
 
 // ---- wide kernel: persistent traversal of the compressed 4-wide tree (wide_bvh.cuh) -------------------
 // One lane per ray, same refill / bounded-round structure as trace_persistent_kernel.  An inner step
-// fetches ONE 64-byte node (two 256-bit loads from the same line), dequantises four child boxes straight
+// fetches ONE 64-byte node (four 128-bit loads from the same line), dequantises four child boxes straight
 // into ray-parameter space (t = q * (cell * inv_dir) + (origin - org) * inv_dir, far planes with the
 // padded inverse direction so that rounding can only enlarge a box), visits the hit children nearest
 // first and pushes the others far-to-near.  Leaves are the binary tree's leaves: same BVH-order triangle
@@ -736,68 +730,34 @@ trace_wide_kernel(TraceArgs<float> a) {
         unsigned char* stage_base = smem_raw + (size_t)a.wide_entries * kTraceBlock * sizeof(uint32_t);
         stager.init(stage_base, threadIdx.x >> 5, lane, a.stage_hits);
     }
-    auto retire = [&] (unsigned long long index, const HitState<float>& h, float tmax) {
-        if (kGather) stager_retire(stager, a.hits, index, make_record(h, tmax, a.prim_ids));
-        else store_hit(a.hits, index, h, tmax, a.prim_ids);
-    };
 
-    unsigned long long chunk_pos = 0, chunk_end = 0;
-    bool exhausted = false;
+    RunCursor run;
     bool has_ray = false;
     unsigned long long ray_index = 0;
     RayCtx<float> r;                   // aux = padded inverse direction (far planes)
     HitState<float> hit;
     float tmax_in = 0.f;
     uint32_t top = 0;
+    auto retire = [&] { retire_ray<float, kGather>(stager, a.hits, ray_index, hit, tmax_in, a.prim_ids); };
+
+    auto draw = [&] (unsigned idle, unsigned rank) {
+        bool got = false;
+        if (!draw_from_run<float, kGather>(run, a, a.chunk_rays, idle, rank, !has_ray, stager, lane, kFull, ray_index, r, got)) return false;
+        if (got && start_ray<float, kGather>(r, hit, tmax_in, stager, ray_index, retire)) {
+            wide_ray_setup(r);
+            top = 0;                                        // wide node 0, inner
+            stack.clear();
+            has_ray = true;
+        }
+        return true;
+    };
 
     uint32_t rounds = 0;
     for (;;) {
-        if (++rounds > a.watchdog) {
-            if (lane == 0) atomicExch(a.status, 1u);
-            return;
-        }
-        unsigned idle = __ballot_sync(kFull, !has_ray);
-        if ((uint32_t)__popc(idle) < a.refill_min) idle = 0u;       // (see trace_persistent_kernel)
-        while (idle != 0u && !exhausted) {
-            if (chunk_pos == chunk_end) {
-                unsigned long long base = 0;
-                if (lane == 0) base = atomicAdd(a.next_ray, (unsigned long long)a.chunk_rays);
-                base = __shfl_sync(kFull, base, 0);
-                if (base >= a.n) { exhausted = true; break; }
-                chunk_pos = base;
-                chunk_end = base + a.chunk_rays < a.n ? base + a.chunk_rays : a.n;
-            }
-            unsigned avail = (unsigned)(chunk_end - chunk_pos);
-            const unsigned want = __popc(idle);
-            if (kGather) {                                  // one staging group = 32 consecutive rays
-                const unsigned in_group = (unsigned)(chunk_pos & 31ull);
-                if (in_group == 0) stager_open(stager, a.hits, chunk_pos >> 5, avail < 32u ? avail : 32u, lane);
-                if (avail > 32u - in_group) avail = 32u - in_group;
-            }
-            const unsigned take = want < avail ? want : avail;
-            const unsigned rank = __popc(idle & lt_mask);
-            if (!has_ray && rank < take) {
-                ray_index = chunk_pos + rank;
-                if (a.order) ray_index = a.order[ray_index];
-                load_ray(a.rays, ray_index, r);
-                tmax_in = r.tmax;
-                hit.slot = kInvalidId; hit.t = r.tmax; hit.u = 0.f; hit.v = 0.f;
-                if (kGather) stager.tag = stager.tag_for(ray_index);
-                if (ray_interval_is_nan(r)) {
-                    retire(ray_index, hit, tmax_in);
-                } else {
-                    wide_ray_setup(r);
-                    top = 0;                                    // wide node 0, inner
-                    stack.clear();
-                    has_ray = true;
-                }
-            }
-            chunk_pos += take;
-            if (kGather) stager_account(stager, a.hits, lane);
-            idle = __ballot_sync(kFull, !has_ray);
-        }
+        if (watchdog_fired(rounds, a.watchdog, a.status, lane)) return;
+        refill_lanes<float, kGather>(has_ray, run, kFull, a.refill_min, lt_mask, kFull, stager, a.hits, lane, draw);
         if (__ballot_sync(kFull, has_ray) == 0u) {
-            if (exhausted) break;
+            if (run.exhausted) break;
             continue;
         }
 
@@ -819,7 +779,7 @@ trace_wide_kernel(TraceArgs<float> a) {
                 }
                 if (!wide_step<kAny>(w, r, top, stack)) { has_ray = false; break; }
             }
-            if (!has_ray) retire(ray_index, hit, tmax_in);
+            if (!has_ray) retire();
         }
         __syncwarp();
 
@@ -827,7 +787,7 @@ trace_wide_kernel(TraceArgs<float> a) {
         if (has_ray && index_count(top) != 0) {
             leaf_step<float>(a.tris, a.prim_ids, true, top, r, hit, nullptr);
             if ((kAny && hit.slot != kInvalidId) || !stack.try_pop(top)) {
-                retire(ray_index, hit, tmax_in);
+                retire();
                 has_ray = false;
             }
         }
@@ -931,46 +891,52 @@ int launch_persistent(KernelT kernel, const TraceArgs<T>& args, size_t smem, uns
     return 0;
 }
 
-template <typename T, bool kAny>
-int launch_wide(const TraceArgs<T>& args, bool gather, int device, cudaStream_t stream) {
-    if constexpr (sizeof(T) == 4) {
-        const size_t smem = (size_t)args.wide_entries * kTraceBlock * sizeof(uint32_t);
-        if (gather) return launch_persistent(trace_wide_kernel<kAny, true>, args, smem + stage_smem_bytes<T>(), 32, device, stream);
-        return launch_persistent(trace_wide_kernel<kAny, false>, args, smem, 32, device, stream);
-    } else {
-        set_error("trace: the wide kernel is float-only");
-        return -1;
-    }
-}
-
+// One switch over the kernel the plan chose.  staged: gather mode with warp-aggregated hit stores (one bulk copy per 32
+// records and rank, or ONE to the multicast address); otherwise records leave with one store per record and sink.
 template <typename T, bool kAny, bool kRobust>
-int launch(const TraceArgs<T>& args, bool simple, bool stats, bool gather, int device, cudaStream_t stream) {
+int launch(TraceKernel kernel, const TraceArgs<T>& args, bool staged, int device, cudaStream_t stream) {
     using U = typename Real<T>::UInt;
-    const size_t smem = (size_t)args.stack_entries * kTraceBlock * sizeof(U);
+    size_t smem = (size_t)args.stack_entries * kTraceBlock * sizeof(U);
     if (smem > 200 * 1024) { set_error("trace: tree too deep for the shared-memory stack"); return -1; }
-    if (stats || simple) {
+    const size_t stage = staged ? stage_smem_bytes<T>() : 0;
+    void (*persistent)(TraceArgs<T>) = nullptr;
+    unsigned rays_per_warp = 32;
+    switch (kernel) {
+    case kKernelSimple:
+    case kKernelStats: {
         const unsigned long long blocks = (args.n + kTraceBlock - 1) / kTraceBlock;
         if (blocks > 0x7FFFFFFFull) { set_error("trace: batch too large for one launch"); return -1; }
-        if (stats) {
-            if (configure_smem(trace_simple_kernel<T, kAny, kRobust, true>, smem)) return -1;
-            trace_simple_kernel<T, kAny, kRobust, true><<<(unsigned)blocks, kTraceBlock, smem, stream>>>(args);
-        } else {
-            if (configure_smem(trace_simple_kernel<T, kAny, kRobust, false>, smem)) return -1;
-            trace_simple_kernel<T, kAny, kRobust, false><<<(unsigned)blocks, kTraceBlock, smem, stream>>>(args);
-        }
-    } else if (args.variant == 3) {
-        if (launch_wide<T, kAny>(args, gather, device, stream)) return -1;
-    } else if (args.variant == 2) {
-        if (launch_persistent(trace_pair_kernel<T, kAny, kRobust>, args, smem / 2, 16, device, stream)) return -1;   // one stack per lane pair
-    } else {
-        const size_t tma = args.use_tma ? tma_smem_bytes<T>() : 0, stage = gather ? stage_smem_bytes<T>() : 0;
-        int rc;
-        if (args.use_tma) rc = gather ? launch_persistent(trace_persistent_kernel<T, kAny, kRobust, true, true>, args, smem + tma + stage, 32, device, stream)
-                                      : launch_persistent(trace_persistent_kernel<T, kAny, kRobust, true, false>, args, smem + tma, 32, device, stream);
-        else              rc = gather ? launch_persistent(trace_persistent_kernel<T, kAny, kRobust, false, true>, args, smem + stage, 32, device, stream)
-                                      : launch_persistent(trace_persistent_kernel<T, kAny, kRobust, false, false>, args, smem, 32, device, stream);
-        if (rc) return -1;
+        void (*simple)(TraceArgs<T>) = kernel == kKernelStats ? trace_simple_kernel<T, kAny, kRobust, true>
+                                                              : trace_simple_kernel<T, kAny, kRobust, false>;
+        if (configure_smem(simple, smem)) return -1;
+        simple<<<(unsigned)blocks, kTraceBlock, smem, stream>>>(args);
+        break;
     }
+    case kKernelPersistent:
+        persistent = staged ? trace_persistent_kernel<T, kAny, kRobust, false, true> : trace_persistent_kernel<T, kAny, kRobust, false, false>;
+        smem += stage;
+        break;
+    case kKernelPersistentTma:
+        persistent = staged ? trace_persistent_kernel<T, kAny, kRobust, true, true> : trace_persistent_kernel<T, kAny, kRobust, true, false>;
+        smem += tma_smem_bytes<T>() + stage;
+        break;
+    case kKernelPair:
+        persistent = trace_pair_kernel<T, kAny, kRobust>;
+        smem /= 2;                                          // one stack per lane pair
+        rays_per_warp = 16;
+        break;
+    case kKernelWide:
+        if constexpr (sizeof(T) == 4) {
+            persistent = staged ? trace_wide_kernel<kAny, true> : trace_wide_kernel<kAny, false>;
+            smem = (size_t)args.wide_entries * kTraceBlock * sizeof(uint32_t) + stage;
+            break;
+        }
+        [[fallthrough]];
+    default:
+        set_error("trace: no such kernel for this precision");
+        return -1;
+    }
+    if (persistent && launch_persistent(persistent, args, smem, rays_per_warp, device, stream)) return -1;
     BVH_CUDA_TRY(cudaGetLastError());
     return 0;
 }
@@ -996,20 +962,36 @@ int trace_rays(const DeviceBvh<T>& bvh, const DevRay<T>* d_rays, DevHit<T>* d_hi
             args.hits.multicast = static_cast<DevHit<T>*>(gather->multicast) + gather->offset;
         }
     } else if (!d_hits) { set_error("trace: no hit array"); return -1; }
+    const Tunables& tun = tunables();
+    TraceRequest request { flags, d_ray_stats != nullptr, sizeof(T) == 4, bvh.wide != nullptr || !bvh.wide_unavailable,
+                           gather != nullptr, (unsigned long long)n, tun.variant.load(), tun.use_wide.load(),
+                           tun.refill_min.load(), tun.inner_budget.load(), tun.wide_budget.load() };
+    TracePlan plan = plan_trace(request);
+    if (plan.kernel == kKernelWide && !bvh.wide) {              // the wide tree is derived on first use
+        if (rebuild_wide(const_cast<DeviceBvh<T>&>(bvh), stream, true)) return -1;
+        request.wide_tree = bvh.wide != nullptr;
+        plan = plan_trace(request);
+    }
+    bvh.last_kernel = plan.kernel;
     args.ray_stats = d_ray_stats;
     args.lowest_id = (flags & kTraceLastVisited) ? 0 : 1;
     uint32_t entries = bvh.depth + 2;                           // depth + 1 pending far children at most, + the sentinel
     {                                                           // (an entry is one 512-byte row of the block: any count keeps the alignment)
-        const uint32_t r = (uint32_t)tunables().stack_round.load();
+        const uint32_t r = (uint32_t)tun.stack_round.load();
         entries = (entries + r - 1u) / r * r;
     }
     if (entries < 16) entries = 16;
     args.stack_entries = entries;
-    args.next_ray = nullptr;
-    args.inner_budget = tunables().inner_budget.load();
-    args.refill_min = tunables().refill_min.load();
+    args.wide = nullptr; args.wide_entries = 0;
+    if (plan.kernel == kKernelWide) {
+        args.wide = bvh.wide;
+        const uint32_t e = 3 * bvh.wide_depth + 3;              // (+ the sentinel entry)
+        args.wide_entries = (e + 1u) & ~1u;
+    }
+    args.inner_budget = plan.inner_budget;
+    args.refill_min = plan.refill_min;
     {   // a warp's private run of consecutive rays: as long as the batch allows with ~8 runs per resident warp (tail balance)
-        uint32_t run = tunables().chunk_rays.load();
+        uint32_t run = tun.chunk_rays.load();
         int sm_count = 132;
         BVH_CUDA_TRY(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, bvh.device));
         const unsigned long long fair = n / ((unsigned long long)sm_count * 32ull * 8ull);
@@ -1017,28 +999,9 @@ int trace_rays(const DeviceBvh<T>& bvh, const DevRay<T>* d_rays, DevHit<T>* d_hi
         run &= ~31u;
         args.chunk_rays = run < 32u ? 32u : run;
     }
-    args.watchdog = tunables().watchdog.load();
+    args.watchdog = tun.watchdog.load();
     args.full_mask = 0xFFFFFFFFu;
-    args.stage_hits = tunables().gather_staging.load() != 0;
-    args.variant = (flags & kTracePair) ? 2 : ((flags & (kTraceNoTma | kTraceTma)) ? 0 : tunables().variant.load());
-    // the wide (compressed 4-wide) path: float, canonical tie-break, fast slab test, no statistics
-    args.wide = nullptr; args.wide_entries = 0;
-    if constexpr (sizeof(T) == 4) {
-        const bool explicit_binary = (flags & (kTracePair | kTraceNoTma | kTraceTma | kTraceSimple)) != 0;
-        const bool order_sensitive = (flags & (kTraceLastVisited | kTraceRobust)) != 0 || d_ray_stats != nullptr;
-        const bool want_wide = !order_sensitive && ((flags & kTraceWide) || (!explicit_binary && (tunables().use_wide.load() > 0)));
-        if (want_wide && !bvh.wide && !bvh.wide_unavailable) {      // derived on first use
-            if (rebuild_wide(const_cast<DeviceBvh<T>&>(bvh), stream, true)) return -1;
-        }
-        if (bvh.wide && want_wide) {
-            args.wide = bvh.wide;
-            uint32_t e = 3 * bvh.wide_depth + 3;                // (+ the sentinel entry)
-            args.wide_entries = (e + 1u) & ~1u;
-            args.variant = 3;
-        }
-    }
-    args.use_tma = (flags & kTraceTma) ? true : ((flags & kTraceNoTma) ? false : tunables().variant.load() == 1);
-    const bool simple = (flags & kTraceSimple) != 0, stats = d_ray_stats != nullptr;
+    args.stage_hits = tun.gather_staging.load() != 0;
     if (!bvh.scratch) {
         void* p = nullptr;
         if (device_alloc(&p, 2 * sizeof(unsigned long long), stream)) return -1;
@@ -1047,33 +1010,14 @@ int trace_rays(const DeviceBvh<T>& bvh, const DevRay<T>* d_rays, DevHit<T>* d_hi
     }
     args.next_ray = bvh.scratch;
     args.status = reinterpret_cast<uint32_t*>(bvh.scratch + 1);
-    // ray reordering: persistent kernels without bulk-copied ray chunks (a chunk is no longer contiguous); not in
-    // gather mode (its staging groups are runs of consecutive ray indices), not for the diagnostic kernels
     RayOrderScratch order_scratch(stream);
     args.order = nullptr;
-    if ((flags & kTraceSortRays) && !gather && !simple && !stats && args.variant != 2 && n >= (1u << 16) && n < 0xFFFFFFFFull) {
-        if (make_ray_order(bvh, d_rays, (uint32_t)n, order_scratch, &args.order, stream)) return -1;
-        args.use_tma = false;
-    }
-    int rc;
-    const bool any = (flags & kTraceAnyHit) != 0, robust = (flags & kTraceRobust) != 0;
-    // gather mode: the kernel variants with warp-aggregated hit stores when staging is on (one bulk copy per 32 records and
-    // rank, or ONE bulk copy to the multicast address); otherwise the plain variants deliver the records with store_hit()
-    // (one store per record and rank / one multimem store) and carry none of the staging code
+    if (plan.sort_rays && make_ray_order(bvh, d_rays, (uint32_t)n, order_scratch, &args.order, stream)) return -1;
     const bool staged = gather != nullptr && args.stage_hits;
-    // refill threshold and inner budget, 0 = auto (DESIGN.md §3, measured on the H100): closest-hit rays in the binary
-    // persistent kernel run best with 14 / 4; any-hit rays and the lane-pair and wide kernels with 8 / 8
-    const bool closest_binary = !any && (args.variant == 0 || args.variant == 1);
-    if (args.refill_min == 0) args.refill_min = closest_binary ? 14u : 8u;
-    if (args.inner_budget == 0) args.inner_budget = closest_binary ? 4u : 8u;
-    if (args.variant == 3) args.inner_budget = tunables().wide_budget.load();
-    bvh.last_kernel = stats ? kKernelStats : simple ? kKernelSimple : args.variant == 3 ? kKernelWide : args.variant == 2 ? kKernelPair
-                    : args.use_tma ? kKernelPersistentTma : kKernelPersistent;
-    if (any) rc = robust ? launch<T, true, true>(args, simple, stats, staged, bvh.device, stream)
-                         : launch<T, true, false>(args, simple, stats, staged, bvh.device, stream);
-    else     rc = robust ? launch<T, false, true>(args, simple, stats, staged, bvh.device, stream)
-                         : launch<T, false, false>(args, simple, stats, staged, bvh.device, stream);
-    return rc;
+    if (flags & kTraceAnyHit) return (flags & kTraceRobust) ? launch<T, true, true>(plan.kernel, args, staged, bvh.device, stream)
+                                                            : launch<T, true, false>(plan.kernel, args, staged, bvh.device, stream);
+    return (flags & kTraceRobust) ? launch<T, false, true>(plan.kernel, args, staged, bvh.device, stream)
+                                  : launch<T, false, false>(plan.kernel, args, staged, bvh.device, stream);
 }
 
 template <typename T> int check_trace_status(const DeviceBvh<T>& bvh, cudaStream_t stream) {

@@ -76,10 +76,10 @@ __device__ __forceinline__ void ldg256_node(const void* p, unsigned long long (&
 #endif
 
 #if defined(__CUDA_ARCH__)
-// sm_100 has 256-bit global loads (SASS LDG.E.256): a node is ONE load, a sibling pair two, from one
-// naturally aligned 64-byte (float) / 128-byte (double) block, through the read-only path.  Halving the
-// number of load instructions matters because with divergent rays every load costs one L1 tag lookup per
-// distinct line touched by the warp (profiles/: the traversal is L1-tag bound, not DRAM bound).
+// A sibling pair is one naturally aligned 64-byte (float) / 128-byte (double) block, read through the read-only path:
+// on sm_90a a 32-byte float node is two 128-bit loads (LDG.E.128), a pair four.  The number of load instructions
+// matters because with divergent rays every load costs one L1 wavefront per distinct piece the warp addresses (the
+// traversal is bound by the L1 data pipe, not by DRAM; DESIGN.md §3).
 __device__ __forceinline__ void load_pair(const DevNode<float>* __restrict__ p, NodePair<float>& o) {
     uint32_t a[8], b[8];
     ldg256_node(p, a);

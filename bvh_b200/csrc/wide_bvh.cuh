@@ -2,8 +2,8 @@
 // path (float only).
 //
 // Why it exists: with divergent rays the binary traversal is bound by the L1 data pipe — every lane's
-// fetch of a 64-byte sibling pair costs two wavefronts (profiles/: l1tex__data_pipe_lsu_wavefronts at
-// ~87 % of peak at 2.6 Grays/s).  A 4-wide node with 8-bit quantised child boxes is ALSO 64 bytes, but one
+// fetch of a 64-byte sibling pair costs two wavefronts (l1tex__data_pipe_lsu_wavefronts measured at ~87 % of
+// peak at 2.6 Grays/s on an earlier GPU).  A 4-wide node with 8-bit quantised child boxes is ALSO 64 bytes, but one
 // step through it replaces about two binary steps, so a ray needs roughly half as many wavefronts.
 //
 // It is derived on the device from the reference-layout binary tree (which stays authoritative: host
@@ -20,7 +20,7 @@
 
 namespace bvhb200 {
 
-// One 4-wide node: 64 bytes, 64-byte aligned (two 256-bit loads from one line).
+// One 4-wide node: 64 bytes, 64-byte aligned (four 128-bit loads from one line).
 //   origin[3]            the node's box minimum
 //   exp[3]               biased IEEE exponents: cell size on axis a = 2^(exp[a]-127); 0 means a flat axis
 //   count                number of used child slots (1..4)

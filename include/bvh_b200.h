@@ -93,12 +93,13 @@ BVH_API void bvh_host_free(void* ptr);
  * in it (rebuilds never go back to the driver); this hands the cached blocks of `device` back. */
 BVH_API int bvh_cuda_trim(int device);
 /* Process-wide switches for experiments, A/B measurements and tests (the defaults are the measured best):
- * "morton_bits" 0|30|63, "sah_treelets" -1|0|1, "hierarchy" 0|64|128|256, "e2e_chunks", "variant" 0|1,
+ * "morton_bits" 0|30|63, "sah_treelets" -1|0|1, "hierarchy" 0|64|128|256, "e2e_chunks", "variant" 0|1 (other values are an error),
  * "use_wide" 0|1, "inner_budget" (unset: auto, <= 0: unbounded), "refill_min" 1..32 (idle lanes a warp waits for
  * before it draws new rays; 0: auto — 14 with inner budget 4 for closest-hit rays, 8 / 8 for any-hit rays and the wide kernel),
  * "chunk_rays" (consecutive rays a warp claims at a time), "wide_budget", "watchdog", "gather_staging" 0|1,
  * "sort_onesweep" 0|1, "treelet_blocks" 2|3|4, "stack_round", "smem_carveout" -1|0..100.  Initial values come from
- * the BVH_B200_<NAME> environment variables, read once when the library is first used; unknown names are an error. */
+ * the BVH_B200_<NAME> environment variables, read once when the library is first used, which are clamped the same way
+ * (a value an option rejects keeps its default); unknown names are an error. */
 BVH_API int bvh_set_option(const char* name, long value);
 /* Subtree reinsertion (reference ReinsertionOptimizer::optimize, reinsertion_optimizer.h:27-30,218-267) on a
  * caller-owned node array in the reference layout: node_count nodes of Node<float|double, dim> (2*dim bounds as
