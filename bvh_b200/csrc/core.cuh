@@ -244,12 +244,12 @@ template <typename T> inline T acc_min(T tf, T t1) { return robust_min(tf, t1); 
 // tmin/tmax fails: node.h:110-115, tri.h:69); callers retire it as a miss without traversing.
 template <typename T> BVH_HD bool ray_interval_is_nan(const RayCtx<T>& r) { return r.tmin != r.tmin || r.tmax != r.tmax; }
 
-// reference node.h:68-88 + make_intersection_result (:105-117).  b = [minx,maxx,miny,maxy,minz,maxz]
-// (kDim = 2: [minx,maxx,miny,maxy], the reference's Node<T, 2>)
-template <typename T, bool kRobust, int kDim = 3> BVH_HD void node_test(const T* b, const RayCtx<T>& r, T& t0, T& t1) {
+// The slab test of node_test over the axes [kFirst, kLast) only, continuing the interval t0, t1 of the axes tested
+// before them (r.tmin, r.tmax before any).  The accumulation only raises t0 and lowers t1, so an interval that is
+// already empty stays empty whatever the remaining axes give: the box is missed.
+template <typename T, bool kRobust, int kFirst, int kLast> BVH_HD void node_test_axes(const T* b, const RayCtx<T>& r, T& t0, T& t1) {
     using R = Real<T>;
-    t0 = r.tmin; t1 = r.tmax;
-    for (int i = 0; i < kDim; ++i) {
+    for (int i = kFirst; i < kLast; ++i) {
         const bool neg = (r.oct >> i) & 1u;
         const T bnear = neg ? b[2 * i + 1] : b[2 * i];       // get_min_bounds(octant), :59-61
         const T bfar  = neg ? b[2 * i] : b[2 * i + 1];       // get_max_bounds(octant), :63-65
@@ -264,6 +264,13 @@ template <typename T, bool kRobust, int kDim = 3> BVH_HD void node_test(const T*
         t0 = acc_max(tn, t0);
         t1 = acc_min(tf, t1);
     }
+}
+
+// reference node.h:68-88 + make_intersection_result (:105-117).  b = [minx,maxx,miny,maxy,minz,maxz]
+// (kDim = 2: [minx,maxx,miny,maxy], the reference's Node<T, 2>)
+template <typename T, bool kRobust, int kDim = 3> BVH_HD void node_test(const T* b, const RayCtx<T>& r, T& t0, T& t1) {
+    t0 = r.tmin; t1 = r.tmax;
+    node_test_axes<T, kRobust, 0, kDim>(b, r, t0, t1);
 }
 
 // Closest-hit bookkeeping while a ray is in flight.  `slot` is the BVH-order primitive index

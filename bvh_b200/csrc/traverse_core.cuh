@@ -97,6 +97,33 @@ __device__ __forceinline__ void load_pair(const DevNode<double>* __restrict__ p,
     o.lb[4] = __longlong_as_double((long long)b[0]); o.lb[5] = __longlong_as_double((long long)b[1]); o.li = b[2];
     o.rb[4] = __longlong_as_double((long long)d[0]); o.rb[5] = __longlong_as_double((long long)d[1]); o.ri = d[2];
 }
+// The two halves of a float node, [minx maxx miny maxy] and [minz maxz index spare], one LDG.E.128 each, for the
+// closest-hit step that loads a child's second half only when its first does not reject it (inner_step).
+// The first halves of both nodes of the pair at p:
+__device__ __forceinline__ void load_first_halves(const DevNode<float>* __restrict__ p, NodePair<float>& o) {
+    uint32_t a[4], b[4];
+#if BVH_NODE_NA
+    asm("ld.global.nc.L1::no_allocate.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+        "ld.global.nc.L1::no_allocate.v4.b32 {%4,%5,%6,%7}, [%8+32];"
+#else
+    asm("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+        "ld.global.nc.v4.b32 {%4,%5,%6,%7}, [%8+32];"
+#endif
+        : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]) : "l"(p));
+    #pragma unroll
+    for (int k = 0; k < 4; ++k) { o.lb[k] = __uint_as_float(a[k]); o.rb[k] = __uint_as_float(b[k]); }
+}
+// The second half of the node at p: b[4], b[5] and its index.
+__device__ __forceinline__ void load_second_half(const DevNode<float>* __restrict__ p, float (&b)[6], uint32_t& index) {
+    uint32_t w0, w1, w2, w3;
+#if BVH_NODE_NA
+    asm("ld.global.nc.L1::no_allocate.v4.b32 {%0,%1,%2,%3}, [%4+16];"
+#else
+    asm("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4+16];"
+#endif
+        : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3) : "l"(p));
+    b[4] = __uint_as_float(w0); b[5] = __uint_as_float(w1); index = w2;
+}
 // One node (for the lane-pair kernel: each lane of a pair fetches one child of the sibling pair).
 __device__ __forceinline__ void load_node(const DevNode<float>* __restrict__ p, float (&b)[6], uint32_t& index) {
     uint32_t a[8];
@@ -155,6 +182,12 @@ template <typename T> inline void load_pair(const DevNode<T>* p, NodePair<T>& o)
     for (int k = 0; k < 6; ++k) { o.lb[k] = p[0].bounds[k]; o.rb[k] = p[1].bounds[k]; }
     o.li = p[0].index; o.ri = p[1].index;
 }
+template <typename T> inline void load_first_halves(const DevNode<T>* p, NodePair<T>& o) {
+    for (int k = 0; k < 4; ++k) { o.lb[k] = p[0].bounds[k]; o.rb[k] = p[1].bounds[k]; }
+}
+template <typename T> inline void load_second_half(const DevNode<T>* p, T (&b)[6], typename Real<T>::UInt& index) {
+    b[4] = p->bounds[4]; b[5] = p->bounds[5]; index = p->index;
+}
 template <typename T> inline void load_tri(const DevTri<T>* p, DevTri<T>& o) { o = *p; }
 #endif
 
@@ -180,11 +213,27 @@ BVH_HD void inner_step(const DevNode<T>* __restrict__ nodes, const RayCtx<T>& r,
     NodePair<T> pair;
     // Device slot = reference index + 1.  An inner node's count bits are 0, so its first child's byte offset is
     // index_first(top) * sizeof(DevNode<T>) = top * (sizeof(DevNode<T>) >> kPrimCountBits): one multiply-add from `top`.
-    load_pair(reinterpret_cast<const DevNode<T>*>(reinterpret_cast<const unsigned char*>(nodes + 1) +
-                                                  (size_t)top * (sizeof(DevNode<T>) >> kPrimCountBits)), pair);
+    const DevNode<T>* p = reinterpret_cast<const DevNode<T>*>(reinterpret_cast<const unsigned char*>(nodes + 1) +
+                                                              (size_t)top * (sizeof(DevNode<T>) >> kPrimCountBits));
     T l0, l1, r0, r1;
-    node_test<T, kRobust>(pair.lb, r, l0, l1);
-    node_test<T, kRobust>(pair.rb, r, r0, r1);
+    if constexpr (sizeof(T) == 4 && !kAny) {
+        // node_test of both children, split after the x and y axes: a child whose x/y interval is already empty is
+        // missed (node_test_axes), so its second half is neither loaded nor tested, and its index is not used below.
+        // Same operations in the same order as node_test, so the same intervals.  On the device the two conditional
+        // loads become predicated LDGs: a lane that skips one issues nothing for it.  Measured on the H100 (DESIGN.md
+        // §3), this is faster for float closest-hit rays only; any-hit and double-precision rays load whole nodes.
+        pair.li = pair.ri = 0;       // (defined on every path: an index loaded on some only lengthens its live range)
+        load_first_halves(p, pair);
+        l0 = r.tmin; l1 = r.tmax; r0 = r.tmin; r1 = r.tmax;
+        node_test_axes<T, kRobust, 0, 2>(pair.lb, r, l0, l1);
+        node_test_axes<T, kRobust, 0, 2>(pair.rb, r, r0, r1);
+        if (l0 <= l1) { load_second_half(p, pair.lb, pair.li); node_test_axes<T, kRobust, 2, 3>(pair.lb, r, l0, l1); }
+        if (r0 <= r1) { load_second_half(p + 1, pair.rb, pair.ri); node_test_axes<T, kRobust, 2, 3>(pair.rb, r, r0, r1); }
+    } else {
+        load_pair(p, pair);
+        node_test<T, kRobust>(pair.lb, r, l0, l1);
+        node_test<T, kRobust>(pair.rb, r, r0, r1);
+    }
     const bool hit_left = l0 <= l1, hit_right = r0 <= r1;
     // Same decisions as the reference's nested branches (bvh.h:167-181), written as selects: on the device the lanes of a
     // warp take all four outcomes at once, and one predicated path costs fewer issue slots than four divergent ones.
