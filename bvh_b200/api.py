@@ -103,6 +103,8 @@ def lib() -> C.CDLL:
         f("set_triangles").argtypes = [P, P, SZ, U]
         f("refit_triangles").restype = C.c_int
         f("refit_triangles").argtypes = [P, P, SZ, U]
+        f("refit_boxes").restype = C.c_int
+        f("refit_boxes").argtypes = [P, P, SZ, U]
         f("intersect_rays").restype = C.c_int
         f("intersect_rays").argtypes = [P, P, SZ, P, U]
         f("intersect_rays_gather").restype = C.c_int
@@ -252,6 +254,20 @@ class Bvh:
         if isinstance(vertices, np.ndarray):
             vertices = np.ascontiguousarray(vertices, dtype=self.dtype)
         if self._f("refit_triangles")(self.handle, _addr(vertices), n, flags):
+            raise BvhError(last_error())
+
+    def refit_boxes(self, bboxes, flags: int = 0) -> None:
+        """``bvhNN_refit_boxes`` (include/bvh_b200_device.h): GPU refit from per-primitive boxes, ``(n, 6)`` as
+        ``min3, max3`` in the original primitive order (or a device address with ``flags=DEVICE_POINTERS``, holding
+        ``prim_count`` boxes).  Topology and attached triangles are unchanged."""
+        if isinstance(bboxes, np.ndarray):
+            if bboxes.ndim != 2 or bboxes.shape[1] != 6:
+                raise ValueError(f"bboxes must be (n, 6) as min3, max3, not {bboxes.shape}")
+            bboxes = np.ascontiguousarray(bboxes, dtype=self.dtype)
+            n = bboxes.shape[0]
+        else:
+            n = self.prim_count
+        if self._f("refit_boxes")(self.handle, _addr(bboxes), n, flags):
             raise BvhError(last_error())
 
     def destroy(self) -> None:

@@ -838,6 +838,29 @@ BVH_EXPORT void bvh_thread_pool_destroy(struct bvh_thread_pool* pool) { delete p
         BVH_CUDA_TRY(cudaStreamSynchronize(h->stream));                                                            \
         return 0;                                                                                                  \
     }                                                                                                              \
+    BVH_EXPORT int bvh##S##_refit_boxes(struct bvh##S* bvh, const struct bvh_bbox##S* bboxes, size_t prim_count,   \
+            unsigned flags) {                                                                                      \
+        auto h = H(T, bvh);                                                                                        \
+        if (!h) { set_error("refit_boxes: null handle"); return -1; }                                              \
+        if (!bboxes) { set_error("refit_boxes: null boxes"); return -1; }                                         \
+        static_assert(sizeof(bvh_bbox##S) == 6 * sizeof(T), "bbox layout: min3, max3");                            \
+        std::lock_guard<std::mutex> lock(h->batch_mutex);                                                          \
+        /* checked before ensure_device, so that a failed call changes nothing on the device */                   \
+        if (h->host_valid ? h->nodes.empty() : !h->device_valid) { set_error("refit_boxes: handle holds no BVH"); return -1; } \
+        if (prim_count != (h->host_valid ? h->prim_ids.size() : (size_t)h->dev.prim_count)) {                     \
+            set_error("refit_boxes: prim_count mismatch"); return -1;                                              \
+        }                                                                                                          \
+        BVH_ON_DEVICE(h->device);                                                                                  \
+        if (ensure_device(*h)) return -1;                                                                          \
+        const bool device_ptrs = (flags & BVH_DEVICE_POINTERS) != 0;                                               \
+        DeviceInput<T> db(h->stream);                                                                              \
+        if (db.set(reinterpret_cast<const T*>(bboxes), 6 * prim_count, device_ptrs)) return -1;                   \
+        if (refit_boxes<T>(h->dev, db.ptr, h->stream)) return -1;                                                  \
+        h->host_valid = false;                   /* the mirror (if any) is stale: re-download on demand */        \
+        h->nodes.clear(); h->prim_ids.clear();                                                                     \
+        if (!device_ptrs) BVH_CUDA_TRY(cudaStreamSynchronize(h->stream));                                          \
+        return 0;                                                                                                  \
+    }                                                                                                              \
     BVH_EXPORT int bvh##S##_intersect_rays(struct bvh##S* bvh, const struct bvh_ray##S* rays, size_t ray_count,    \
             struct bvh_hit##S* hits, unsigned flags) {                                                             \
         return intersect_batch<T>(H(T, bvh), rays, ray_count, hits, nullptr, flags);                               \

@@ -117,6 +117,11 @@ int attach_triangles(DeviceBvh<T>& bvh, const T* d_verts, cudaStream_t stream);
 template <typename T>
 int refit_triangles(DeviceBvh<T>& bvh, const T* d_verts, cudaStream_t stream);
 
+// The same pass with the leaf boxes folded from per-primitive boxes (prim_count x 6: min3, max3, original order); the
+// triangles, if any, are left as they are.  Stream-ordered unless a wide companion tree has to be rebuilt.
+template <typename T>
+int refit_boxes(DeviceBvh<T>& bvh, const T* d_boxes, cudaStream_t stream);
+
 // Writes the tree in the reference's own layout into device buffers the caller copies to the host: node_slots - 1
 // records of Node<T,3> (7 words each) and prim_count 64-bit primitive ids.  The device tree must be dense.
 template <typename T>

@@ -20,6 +20,7 @@
 #include "build_core.cuh"
 #include "engine.h"
 #include "radix_sort.cuh"
+#include "refit_core.cuh"
 #include "treelet_warp.cuh"
 #include "wide_bvh.cuh"
 
@@ -441,73 +442,43 @@ permute_tris_kernel(const T* __restrict__ verts, const uint32_t* __restrict__ pr
     for (int k = 0; k < (int)(sizeof(DevTri<T>) / 16); ++k) d[k] = s[k];
 }
 
-// ---- GPU refit (reference Bvh::refit, bvh.h:184-218, with the leaf function recomputing the leaf
-// boxes from moved vertices — what an animation loop does every frame) ----------------------------------
+// ---- GPU refit (reference Bvh::refit, bvh.h:184-218, with a leaf function that gives the leaf boxes: from moved
+// vertices or from the caller's per-primitive boxes — what an animation loop does every frame).  The pass itself is
+// refit_core.cuh. ----------------------------------------------------------------------------------------------
 // K_r1: parent[child slot] = parent slot, for every inner node.
 template <typename T>
 __global__ void __launch_bounds__(kBlock)
 refit_parents_kernel(const DevNode<T>* __restrict__ nodes, size_t slots, uint32_t* __restrict__ parent, int* __restrict__ flags) {
     const size_t i = (size_t)blockIdx.x * kBlock + threadIdx.x + 1;
-    if (i >= slots) return;
-    flags[i] = 0;
-    const auto index = nodes[i].index;
-    if (index_count(index) == 0) {
-        const size_t first = (size_t)index_first(index) + 1;          // device slot of the left child
-        if (first + 1 < slots) { parent[first] = (uint32_t)i; parent[first + 1] = (uint32_t)i; }
-    }
-    if (i == 1) parent[1] = 0;
+    if (i < slots) refit_link(nodes, slots, i, parent, flags);
 }
 
-// K_r2: one thread per leaf slot: box of its triangles (tri.h:24, in BVH order), BVH-order PrecomputedTri
-// (tri.h:35-37), then climb; the second child to arrive unions the two boxes in the reference's order
-// (left.get_bbox().extend(right.get_bbox()), bvh.h:213-217).
-template <typename T>
+// K_r2: one thread per leaf slot: leaf box, then the climb.
+template <typename T, typename BoxOf>
 __global__ void __launch_bounds__(kBlock)
 refit_leaves_kernel(DevNode<T>* __restrict__ nodes, size_t slots, const uint32_t* __restrict__ parent, int* __restrict__ flags,
-                    const T* __restrict__ verts, const uint32_t* __restrict__ prim_ids, DevTri<T>* __restrict__ tris) {
-    using R = Real<T>;
+                    const uint32_t* __restrict__ prim_ids, BoxOf box_of) {
     const size_t i = (size_t)blockIdx.x * kBlock + threadIdx.x + 1;
-    if (i >= slots) return;
-    const auto index = nodes[i].index;
-    const uint32_t count = index_count(index);
-    if (count == 0) return;
-    const uint32_t first = (uint32_t)index_first(index);
-    T bmin[3] = { R::max(), R::max(), R::max() };
-    T bmax[3] = { R::neg(R::max()), R::neg(R::max()), R::neg(R::max()) };
-    for (uint32_t k = first; k < first + count; ++k) {
-        const uint32_t id = prim_ids[k];
+    if (i < slots) refit_from_leaf(nodes, i, parent, flags, prim_ids, box_of);
+}
+
+// Leaf boxes from triangles (tri.h:24); also stores the BVH-order PrecomputedTri of slot k (tri.h:35-37).
+template <typename T> struct TriangleSource {
+    const T* verts;
+    DevTri<T>* tris;
+    __device__ __forceinline__ void operator()(uint32_t k, uint32_t id, T bmin[3], T bmax[3]) const {
         T v[9];
         #pragma unroll
         for (int j = 0; j < 9; ++j) v[j] = __ldg(verts + 9 * (size_t)id + j);
-        T tmin[3], tmax[3], c[3];
-        tri_bounds_center(v, tmin, tmax, c);
-        #pragma unroll
-        for (int a = 0; a < 3; ++a) { bmin[a] = robust_min(bmin[a], tmin[a]); bmax[a] = robust_max(bmax[a], tmax[a]); }
+        T c[3];
+        tri_bounds_center(v, bmin, bmax, c);
         const DevTri<T> t = precompute_tri(v);
         const uint4* s = reinterpret_cast<const uint4*>(&t);
         uint4* d = reinterpret_cast<uint4*>(tris + k);
         #pragma unroll
         for (int j = 0; j < (int)(sizeof(DevTri<T>) / 16); ++j) d[j] = s[j];
     }
-    write_node(nodes + i, bmin, bmax, index);
-    size_t node = i;
-    while (node != 1) {
-        const size_t p = parent[node];
-        if (p == 0) return;                                            // dead slot (collapsed subtree)
-        cuda::atomic_ref<int, cuda::thread_scope_device> flag(flags[p]);
-        if (flag.fetch_add(1, cuda::memory_order_acq_rel) == 0) return; // the sibling will carry on
-        const size_t left = (size_t)index_first(nodes[p].index) + 1;
-        const DevNode<T> l = DeviceSync::load(nodes + left), r = DeviceSync::load(nodes + left + 1);
-        T pmin[3], pmax[3];
-        #pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            pmin[a] = robust_min(l.bounds[2 * a], r.bounds[2 * a]);
-            pmax[a] = robust_max(l.bounds[2 * a + 1], r.bounds[2 * a + 1]);
-        }
-        write_node(nodes + p, pmin, pmax, nodes[p].index);
-        node = p;
-    }
-}
+};
 
 // ---- collapse of the binary tree into the compressed 4-wide tree (wide_bvh.cuh) ------------------------
 // Level-synchronous: the frontier of level L holds (device slot of a binary inner node, index of the wide
@@ -623,6 +594,19 @@ template <typename T> int make_wide_tree(DeviceBvh<T>& bvh, cudaStream_t stream,
     BVH_CUDA_TRY(cudaStreamSynchronize(stream));
     finish_wide_tree(bvh, host_counters, rounds, stream);
     return 0;
+}
+
+// Both refit kernels on the stream, then the wide companion tree rebuilt when the handle has one (which synchronises).
+template <typename T, typename BoxOf> int refit_with(DeviceBvh<T>& bvh, const BoxOf& box_of, cudaStream_t stream) {
+    Scratch scratch(stream);
+    uint32_t* parent; int* flags;
+    if (scratch.alloc(&parent, bvh.node_slots) || scratch.alloc(&flags, bvh.node_slots)) return -1;
+    BVH_CUDA_TRY(cudaMemsetAsync(parent, 0, bvh.node_slots * sizeof(uint32_t), stream));
+    const unsigned blocks = (unsigned)((bvh.node_slots + kBlock - 1) / kBlock);
+    refit_parents_kernel<T><<<blocks, kBlock, 0, stream>>>(bvh.nodes, bvh.node_slots, parent, flags);
+    refit_leaves_kernel<T><<<blocks, kBlock, 0, stream>>>(bvh.nodes, bvh.node_slots, parent, flags, bvh.prim_ids, box_of);
+    BVH_CUDA_TRY(cudaGetLastError());
+    return make_wide_tree(bvh, stream);
 }
 
 template <typename T, typename K>
@@ -787,15 +771,13 @@ template <typename T>
 int refit_triangles(DeviceBvh<T>& bvh, const T* d_verts, cudaStream_t stream) {
     if (!bvh.nodes) { set_error("refit: no BVH"); return -1; }
     if (!bvh.tris && device_alloc(reinterpret_cast<void**>(&bvh.tris), (size_t)bvh.prim_count * sizeof(DevTri<T>), stream)) return -1;
-    Scratch scratch(stream);
-    uint32_t* parent; int* flags;
-    if (scratch.alloc(&parent, bvh.node_slots) || scratch.alloc(&flags, bvh.node_slots)) return -1;
-    BVH_CUDA_TRY(cudaMemsetAsync(parent, 0, bvh.node_slots * sizeof(uint32_t), stream));
-    const unsigned blocks = (unsigned)((bvh.node_slots + kBlock - 1) / kBlock);
-    refit_parents_kernel<T><<<blocks, kBlock, 0, stream>>>(bvh.nodes, bvh.node_slots, parent, flags);
-    refit_leaves_kernel<T><<<blocks, kBlock, 0, stream>>>(bvh.nodes, bvh.node_slots, parent, flags, d_verts, bvh.prim_ids, bvh.tris);
-    BVH_CUDA_TRY(cudaGetLastError());
-    return make_wide_tree(bvh, stream);
+    return refit_with(bvh, TriangleSource<T>{ d_verts, bvh.tris }, stream);
+}
+
+template <typename T>
+int refit_boxes(DeviceBvh<T>& bvh, const T* d_boxes, cudaStream_t stream) {
+    if (!bvh.nodes) { set_error("refit_boxes: no BVH"); return -1; }
+    return refit_with(bvh, BoxSource<T>{ d_boxes }, stream);
 }
 
 template <typename T>
@@ -827,6 +809,8 @@ template int rebuild_wide<float>(DeviceBvh<float>&, cudaStream_t, bool);
 template int rebuild_wide<double>(DeviceBvh<double>&, cudaStream_t, bool);
 template int refit_triangles<float>(DeviceBvh<float>&, const float*, cudaStream_t);
 template int refit_triangles<double>(DeviceBvh<double>&, const double*, cudaStream_t);
+template int refit_boxes<float>(DeviceBvh<float>&, const float*, cudaStream_t);
+template int refit_boxes<double>(DeviceBvh<double>&, const double*, cudaStream_t);
 template int export_reference_arrays<float>(const DeviceBvh<float>&, void*, unsigned long long*, cudaStream_t);
 template int export_reference_arrays<double>(const DeviceBvh<double>&, void*, unsigned long long*, cudaStream_t);
 template void release<float>(DeviceBvh<float>&, cudaStream_t);
