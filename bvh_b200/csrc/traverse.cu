@@ -1,7 +1,7 @@
 // bvh_b200/csrc/traverse.cu — batched closest-hit / any-hit ray traversal kernels (sm_90a).
 //
 // Replaces the caller-side ray loop around Bvh::intersect (reference bvh.h:159-182 driven by
-// test/benchmark.cpp:340-393 / c_api/bvh_impl.h:235-250) with two kernels over a whole ray batch:
+// test/benchmark.cpp:340-393 / c_api/bvh_impl.h:235-250) with kernels over a whole ray batch:
 //
 //   trace_persistent_kernel  persistent warps.  Each warp owns private runs of consecutive rays claimed with one
 //                            global atomicAdd per run; idle lanes are refilled from the run by ballot + prefix rank
@@ -13,11 +13,14 @@
 //                            a warp's accesses never bank-conflict.  kTma: the run's rays staged into shared memory by
 //                            bulk async copies instead of streaming loads; kGather: hit records delivered to every
 //                            rank's gathered array by warp-staged bulk copies (fused multi-GPU gather).
+//   trace_wide_kernel        the same rounds (run_rounds, shared with trace_persistent_kernel) over the compressed
+//                            4-wide tree of wide_bvh.cuh.
+//   trace_pair_kernel        two lanes per ray, one child box each; the same ray feed, its own round loop.
 //   trace_simple_kernel      one thread per ray, same stack machine; also the statistics variant that
 //                            counts inner steps / leaves / triangle tests per ray (the reference's
 //                            InnerFn hook, bvh.h:168) which defines the algorithmic bytes of DESIGN.md.
 //
-// Both kernels execute the reference's per-ray algorithm exactly (traverse_core.cuh), so on the same
+// The binary-tree kernels execute the reference's per-ray algorithm exactly (traverse_core.cuh), so on the same
 // tree they visit nodes in the same order as the CPU code and produce bit-identical ids, t, u, v.
 #include <cstdio>
 #include <cstdlib>
@@ -438,6 +441,38 @@ template <typename T> __host__ __device__ constexpr size_t tma_smem_bytes() {
     return (size_t)(kTraceBlock / 32) * 2 * kTmaChunkRays * sizeof(DevRay<T>) + (size_t)(kTraceBlock / 32) * 2 * 8;
 }
 
+// The rounds of a persistent kernel, until the batch has no rays left.  A round: the watchdog (`rounds`: the count to
+// start from); refill_lanes through draw(idle, rank); the kernel's inner phase inner(), which retires the rays it
+// finishes; the leaf phase, which retires a ray on an any-hit hit or an empty stack.  `mask` is the member mask of every
+// warp primitive.  The lane's ray state (has_ray, top, r, hit, stack) belongs to the kernel; retire() stores its record.
+template <typename T, bool kAny, bool kGather, typename U, typename Stack, typename Draw, typename Retire, typename Inner>
+__device__ __forceinline__ void run_rounds(const TraceArgs<T>& a, const RunCursor& run, bool& has_ray, U& top, RayCtx<T>& r,
+                                           HitState<T>& hit, Stack& stack, HitStager<T>& stager, unsigned mask, uint32_t rounds,
+                                           unsigned lanes, uint32_t refill_min, unsigned lt_mask, bool lowest_id, unsigned lane,
+                                           Draw&& draw, Retire&& retire, Inner&& inner) {
+    for (;;) {
+        if (watchdog_fired(rounds, a.watchdog, a.status, lane)) return;
+        refill_lanes<T, kGather>(has_ray, run, lanes, refill_min, lt_mask, mask, stager, a.hits, lane, draw);
+        if (__ballot_sync(mask, has_ray) == 0u) {
+            if (run.exhausted) break;                        // nothing in flight and nothing left
+            continue;                                        // (only NaN rays were drawn: refill again)
+        }
+        inner();
+        __syncwarp(mask);
+
+        if (has_ray && index_count(top) != 0) {
+            leaf_step<T>(a.tris, a.prim_ids, lowest_id, top, r, hit, nullptr);
+            if ((kAny && hit.slot != kInvalidId) || !stack.try_pop(top)) {
+                retire();
+                has_ray = false;
+            }
+        }
+        __syncwarp(mask);
+        if (kGather) stager_account(stager, a.hits, lane);
+    }
+    if (kGather && stager.buf && lane == 0) bulk_wait_all();         // the last bulk stores have left shared memory and landed
+}
+
 // Persistent kernel.  kTma = true stages the warp's next ray chunk into shared memory with a bulk
 // asynchronous copy (cp.async.bulk, SASS UBLKCP) signalled through an mbarrier, double-buffered, so
 // that the ray fetch of the refill path never waits on DRAM; kTma = false reads rays with streaming
@@ -545,17 +580,9 @@ trace_persistent_kernel(TraceArgs<T> a) {
         return true;
     };
 
-    uint32_t rounds = 0;
-    for (;;) {
-        if (watchdog_fired(rounds, a.watchdog, a.status, lane)) return;
-        refill_lanes<T, kGather>(has_ray, run, kFull, a.refill_min, lt_mask, kFull, stager, a.hits, lane, draw);
-        if (__ballot_sync(kFull, has_ray) == 0u) {
-            if (run.exhausted) break;                        // nothing in flight and nothing left
-            continue;                                        // (only NaN rays were drawn: refill again)
-        }
-
-        // ---- inner phase: descend until this lane holds a leaf, its ray is finished, or the step
-        //      budget of this round is spent (bounding the wait of lanes that already hold a leaf) ----
+    // inner phase: descend until this lane holds a leaf, its ray is finished, or the step budget of this round is spent
+    // (bounding the wait of lanes that already hold a leaf)
+    auto inner = [&] {
         if (has_ray) {
             uint32_t budget = inner_budget;
             while (index_count(top) == 0 && budget != 0) {                     // (kTraversalDone ends it too)
@@ -567,20 +594,9 @@ trace_persistent_kernel(TraceArgs<T> a) {
                 has_ray = false;
             }
         }
-        __syncwarp();
-
-        // ---- leaf phase ---------------------------------------------------------------------------
-        if (has_ray && index_count(top) != 0) {
-            leaf_step<T>(a.tris, a.prim_ids, lowest_id, top, r, hit, nullptr);
-            if ((kAny && hit.slot != kInvalidId) || !stack.try_pop(top)) {
-                retire();
-                has_ray = false;
-            }
-        }
-        __syncwarp();
-        if (kGather) stager_account(stager, a.hits, lane);
-    }
-    if (kGather && stager.buf && lane == 0) bulk_wait_all();         // the last bulk stores have left shared memory and landed
+    };
+    run_rounds<T, kAny, kGather>(a, run, has_ray, top, r, hit, stack, stager, kFull, 0u, kFull, a.refill_min, lt_mask, lowest_id,
+                                 lane, draw, retire, inner);
 }
 
 // ---- lane-pair kernel ------------------------------------------------------------------------------
@@ -752,18 +768,10 @@ trace_wide_kernel(TraceArgs<float> a) {
         return true;
     };
 
-    uint32_t rounds = 0;
-    for (;;) {
-        if (watchdog_fired(rounds, a.watchdog, a.status, lane)) return;
-        refill_lanes<float, kGather>(has_ray, run, kFull, a.refill_min, lt_mask, kFull, stager, a.hits, lane, draw);
-        if (__ballot_sync(kFull, has_ray) == 0u) {
-            if (run.exhausted) break;
-            continue;
-        }
-
-        // ---- inner phase ----------------------------------------------------------------------------
-        // (Speculative descent — a lane that reaches a leaf puts it aside once and keeps descending — was measured
-        // slower on an earlier GPU and removed: the steps taken before tmax shrinks cost more than the idle lanes they fill.)
+    // inner phase
+    // (Speculative descent — a lane that reaches a leaf puts it aside once and keeps descending — was measured
+    // slower on an earlier GPU and removed: the steps taken before tmax shrinks cost more than the idle lanes they fill.)
+    auto inner = [&] {
         if (has_ray) {
             uint32_t budget = inner_budget;
             while (index_count(top) == 0 && budget != 0) {
@@ -781,20 +789,10 @@ trace_wide_kernel(TraceArgs<float> a) {
             }
             if (!has_ray) retire();
         }
-        __syncwarp();
-
-        // ---- leaf phase -----------------------------------------------------------------------------
-        if (has_ray && index_count(top) != 0) {
-            leaf_step<float>(a.tris, a.prim_ids, true, top, r, hit, nullptr);
-            if ((kAny && hit.slot != kInvalidId) || !stack.try_pop(top)) {
-                retire();
-                has_ray = false;
-            }
-        }
-        __syncwarp();
-        if (kGather) stager_account(stager, a.hits, lane);
-    }
-    if (kGather && stager.buf && lane == 0) bulk_wait_all();
+    };
+    // (plan_trace never chooses this kernel for BVH_TIE_LAST_VISITED: the lowest id wins ties)
+    run_rounds<float, kAny, kGather>(a, run, has_ray, top, r, hit, stack, stager, kFull, 0u, kFull, a.refill_min, lt_mask, true, lane,
+                                     draw, retire, inner);
 }
 
 
