@@ -86,6 +86,8 @@ def lib() -> C.CDLL:
         f("build").argtypes = [P, P, P, SZ, C.POINTER(BuildConfig)]
         f("build_triangles").restype = P
         f("build_triangles").argtypes = [P, SZ, C.POINTER(BuildConfig), U]
+        f("build_boxes").restype = P
+        f("build_boxes").argtypes = [P, P, SZ, C.POINTER(BuildConfig), U]
         f("destroy").argtypes = [P]
         f("get_node").restype = P
         f("get_node").argtypes = [P, SZ]
@@ -240,6 +242,29 @@ class Bvh:
         bvh = cls(h, dtype)
         bvh._keep = vertices
         return bvh
+
+    @classmethod
+    def build_boxes(cls, bboxes, centers, count: int | None = None, dtype=None, quality=None,
+                    min_leaf_size=None, max_leaf_size=None, flags: int = 0) -> "Bvh":
+        """``bvhNN_build_boxes`` (include/bvh_b200_device.h): ``bboxes`` ``(n, 6)`` as ``min3, max3`` and ``centers``
+        ``(n, 3)``, or two device addresses with ``flags=DEVICE_POINTERS`` plus ``count`` and ``dtype``.  The same tree
+        as :meth:`build` on the same values."""
+        if isinstance(bboxes, np.ndarray) != isinstance(centers, np.ndarray):
+            raise ValueError("bboxes and centers must both be arrays or both be device addresses")
+        if isinstance(bboxes, np.ndarray):
+            if bboxes.ndim != 2 or bboxes.shape[1] != 6:
+                raise ValueError(f"bboxes must be (n, 6) as min3, max3, not {bboxes.shape}")
+            if centers.shape != (bboxes.shape[0], 3):
+                raise ValueError(f"centers must be ({bboxes.shape[0]}, 3), not {centers.shape}")
+            dtype = bboxes.dtype if dtype is None else dtype
+            bboxes = np.ascontiguousarray(bboxes, dtype=dtype)
+            centers = np.ascontiguousarray(centers, dtype=dtype)
+            count = bboxes.shape[0]
+        elif count is None or dtype is None:
+            raise ValueError("device addresses need count and dtype")
+        h = getattr(lib(), f"bvh{_sfx(dtype)}_build_boxes")(_addr(bboxes), _addr(centers), count,
+                                                            _config(quality, min_leaf_size, max_leaf_size), flags)
+        return cls(h, dtype)
 
     def set_triangles(self, vertices, flags: int = 0) -> None:
         n = vertices.shape[0] if isinstance(vertices, np.ndarray) else self.prim_count

@@ -64,32 +64,44 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
 TEST_KERNELS_SRC = os.path.join(ROOT, "tests", "device_api_kernels.cu")
 TEST_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_api_kernels.so")
+QUERY_KERNELS_SRC = os.path.join(ROOT, "tests", "device_query_kernels.cu")
+QUERY_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_query_kernels.so")
 
 
-def build_device_api_tests(force: bool = False, verbose: bool = False) -> str:
-    """Compiles the device traversal API's test kernels (tests/device_api_kernels.cu) into tests/_build/, linked against
-    the library, with the library's flags (C++20: the file also includes the C++ surface header; x86-64-v3 host code).  Rebuilt when stale and
-    nvcc is present; an existing build is used as it is otherwise."""
-    deps = [TEST_KERNELS_SRC, LIB, os.path.abspath(__file__), os.path.join(ROOT, "include", "bvh", "v2", "cuda", "intersect.cuh"),
+def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
+    """Compiles test kernels that use the device traversal API (src) into tests/_build/ (out), linked against the
+    library, with the library's flags (C++20: the files also include the C++ surface header; x86-64-v3 host code).
+    Rebuilt when stale and nvcc is present; an existing build is used as it is otherwise."""
+    deps = [src, LIB, os.path.abspath(__file__), os.path.join(ROOT, "include", "bvh", "v2", "cuda", "intersect.cuh"),
             os.path.join(ROOT, "include", "bvh", "v2", "b200_surface.h")] + _deps()
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    fresh = os.path.exists(TEST_KERNELS_LIB) and os.path.getmtime(TEST_KERNELS_LIB) >= max(os.path.getmtime(f) for f in deps if os.path.exists(f))
-    if not force and os.path.exists(TEST_KERNELS_LIB) and (fresh or not os.path.exists(nvcc)):
-        return TEST_KERNELS_LIB
-    os.makedirs(os.path.dirname(TEST_KERNELS_LIB), exist_ok=True)
+    fresh = os.path.exists(out) and os.path.getmtime(out) >= max(os.path.getmtime(f) for f in deps if os.path.exists(f))
+    if not force and os.path.exists(out) and (fresh or not os.path.exists(nvcc)):
+        return out
+    os.makedirs(os.path.dirname(out), exist_ok=True)
     flags = ["-std=c++20" if f == "-std=c++17" else f for f in NVCC_FLAGS]
     # the host half runs the C++ surface's Bvh::intersect, whose fast slab test is one FMA only where the target has one
     # (fast_mul_add, FP_FAST_FMAF), as the device's is
     flags += ["-Xcompiler", "-march=x86-64-v3"]
-    cmd = [nvcc, *flags, "-shared",TEST_KERNELS_SRC, "-o", TEST_KERNELS_LIB, "-L", HERE, "-lbvh_c", "-Xlinker", "-rpath,$ORIGIN/../../bvh_b200"]
+    cmd = [nvcc, *flags, "-shared", src, "-o", out, "-L", HERE, "-lbvh_c", "-Xlinker", "-rpath,$ORIGIN/../../bvh_b200"]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0 or verbose:
         sys.stderr.write(res.stdout + res.stderr)
     if res.returncode != 0:
-        raise RuntimeError("nvcc failed on tests/device_api_kernels.cu")
-    return TEST_KERNELS_LIB
+        raise RuntimeError(f"nvcc failed on {os.path.relpath(src, ROOT)}")
+    return out
+
+
+def build_device_api_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_api_kernels.cu: the device traversal API's ray test kernels."""
+    return _build_test_kernels(TEST_KERNELS_SRC, TEST_KERNELS_LIB, force, verbose)
+
+
+def build_device_query_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_query_kernels.cu: the test kernels of DeviceView::traverse_top_down (box overlap, nearest point)."""
+    return _build_test_kernels(QUERY_KERNELS_SRC, QUERY_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

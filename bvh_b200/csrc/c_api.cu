@@ -742,6 +742,14 @@ BVH_EXPORT void bvh_thread_pool_destroy(struct bvh_thread_pool* pool) { delete p
         return reinterpret_cast<bvh##S*>(build_handle<T>(vertices, nullptr, nullptr, prim_count, config,           \
             (flags & BVH_DEVICE_POINTERS) != 0));                                                                  \
     }                                                                                                              \
+    BVH_EXPORT struct bvh##S* bvh##S##_build_boxes(const struct bvh_bbox##S* bboxes, const struct bvh_vec##S* centers, \
+            size_t prim_count, const struct bvh_build_config* config, unsigned flags) {                            \
+        static_assert(sizeof(bvh_bbox##S) == 6 * sizeof(T) && sizeof(bvh_vec##S) == 3 * sizeof(T), "box / centre layout"); \
+        if (!bboxes) { set_error("build_boxes: null boxes"); return nullptr; }                                     \
+        if (!centers) { set_error("build_boxes: null centres"); return nullptr; }                                  \
+        return reinterpret_cast<bvh##S*>(build_handle<T>(nullptr, reinterpret_cast<const T*>(bboxes),              \
+            reinterpret_cast<const T*>(centers), prim_count, config, (flags & BVH_DEVICE_POINTERS) != 0));         \
+    }                                                                                                              \
     BVH_EXPORT void bvh##S##_destroy(struct bvh##S* bvh) { destroy_handle(H(T, bvh)); }                            \
     BVH_EXPORT void bvh##S##_save(const struct bvh##S* bvh, FILE* file) { save_mirror(*HC(T, bvh), file); }        \
     BVH_EXPORT struct bvh##S* bvh##S##_load(FILE* file) { return reinterpret_cast<bvh##S*>(load_mirror<T>(file)); } \

@@ -9,7 +9,8 @@
 // The same code runs in four places: the one-thread-per-ray kernel, the persistent kernel (which
 // splits it into an inner phase and a leaf phase, traverse.cu), the host emulation compiled by
 // g++ for the CPU tests (tests/host_emul.cpp) and, through traverse_top_down with the caller's leaf,
-// the device traversal API (include/bvh/v2/cuda/intersect.cuh).
+// the device traversal API (include/bvh/v2/cuda/intersect.cuh).  traverse_nodes is the same stack machine with the
+// caller's node test instead of the ray's (DeviceView::traverse_top_down).
 #pragma once
 
 #include "core.cuh"
@@ -204,6 +205,20 @@ template <typename U, typename Stack> BVH_HD U pop_or_done(Stack& stack) {
     return stack.try_pop(v) ? v : kTraversalDone<U>;
 }
 
+// The reference's choice after a sibling pair's test (bvh.h:137-149): the near child becomes `top`, the far one is
+// pushed when both are hit (swapped when `swap`), and the stack is popped when both are missed.  Same decisions as the
+// reference's nested branches, written as selects: on the device the lanes of a warp take all four outcomes at once,
+// and one predicated path costs fewer issue slots than four divergent ones.
+template <typename U, typename Stack>
+BVH_HD void descend(bool hit_left, bool hit_right, bool swap, U left_index, U right_index, U& top, Stack& stack) {
+    const bool both = hit_left && hit_right;
+    const bool right_first = both && swap;
+    const U near_index = (hit_left && !right_first) ? left_index : right_index;
+    const U far_index = right_first ? left_index : right_index;
+    if (both) stack.push(far_index);
+    top = (hit_left || hit_right) ? near_index : pop_or_done<U>(stack);
+}
+
 // One inner step (reference bvh.h:132-150 with the lambda of :167-181): `top` (an inner node) becomes the next node to
 // visit, or kTraversalDone when both children were missed and the stack is empty.
 template <typename T, bool kAny, bool kRobust, typename Stack>
@@ -234,15 +249,48 @@ BVH_HD void inner_step(const DevNode<T>* __restrict__ nodes, const RayCtx<T>& r,
         node_test<T, kRobust>(pair.lb, r, l0, l1);
         node_test<T, kRobust>(pair.rb, r, r0, r1);
     }
-    const bool hit_left = l0 <= l1, hit_right = r0 <= r1;
-    // Same decisions as the reference's nested branches (bvh.h:167-181), written as selects: on the device the lanes of a
-    // warp take all four outcomes at once, and one predicated path costs fewer issue slots than four divergent ones.
-    const bool both = hit_left && hit_right;
-    const bool right_first = !kAny && both && l0 > r0;            // ties go left first (`>` at bvh.h:180)
-    const U near_index = (hit_left && !right_first) ? pair.li : pair.ri;
-    const U far_index = right_first ? pair.li : pair.ri;
-    if (both) stack.push(far_index);
-    top = (hit_left || hit_right) ? near_index : pop_or_done<U>(stack);
+    // ties go left first (`>` at bvh.h:180)
+    descend<U>(l0 <= l1, r0 <= r1, !kAny && l0 > r0, pair.li, pair.ri, top, stack);
+}
+
+// Bvh::traverse_top_down with the caller's node test (reference bvh.h:124-157), for queries other than rays: box
+// overlap, point location, nearest-neighbour searches.  The traversal starts at the node index `start` with an empty
+// stack.
+//   node_fn(const DevNode<T>& left, const DevNode<T>& right)  called once per inner node reached, with register copies
+//                                 of its two children; returns anything that unpacks with a structured binding into
+//                                 (hit_left, hit_right, should_swap), each convertible to bool.  should_swap takes
+//                                 effect when both children are hit, whatever kAny is.
+//   leaf_fn(begin, end) -> bool   called on every leaf reached, with its BVH-order primitive range; with kAny a true
+//                                 return ends the traversal.  A leaf `start` is handed to leaf_fn without a node test.
+//   stack                         push(U) and try_pop(U&) (false when empty); it holds at most depth + 1 entries.
+// Each sibling pair is one load_pair: the node test is the caller's, so there is no split of the node load here.
+template <typename T, bool kAny, typename Stack, typename LeafFn, typename NodeFn>
+BVH_HD void traverse_nodes(const DevNode<T>* __restrict__ nodes, typename Real<T>::UInt start, Stack& stack,
+                           LeafFn&& leaf_fn, NodeFn&& node_fn) {
+    using U = typename Real<T>::UInt;
+    U top = start;
+    for (;;) {
+        while (index_count(top) == 0) {
+            // device slot = reference index + 1, the same offset arithmetic as inner_step
+            const DevNode<T>* p = reinterpret_cast<const DevNode<T>*>(reinterpret_cast<const unsigned char*>(nodes + 1) +
+                                                                      (size_t)top * (sizeof(DevNode<T>) >> kPrimCountBits));
+            NodePair<T> pair;
+            load_pair(p, pair);
+            DevNode<T> left, right;
+            for (int k = 0; k < 6; ++k) { left.bounds[k] = pair.lb[k]; right.bounds[k] = pair.rb[k]; }
+            left.index = pair.li; right.index = pair.ri;
+            left.pad = right.pad = 0;
+            const auto [hit_left, hit_right, should_swap] = node_fn(static_cast<const DevNode<T>&>(left),
+                                                                    static_cast<const DevNode<T>&>(right));
+            descend<U>(static_cast<bool>(hit_left), static_cast<bool>(hit_right), static_cast<bool>(should_swap),
+                       pair.li, pair.ri, top, stack);
+        }
+        if (top == kTraversalDone<U>) break;
+        const U first = index_first(top);
+        const bool was_hit = static_cast<bool>(leaf_fn(first, first + (U)index_count(top)));
+        if (kAny && was_hit) break;                             // bvh.h:153-155
+        top = pop_or_done<U>(stack);
+    }
 }
 
 // The triangles [first, first + count) of a leaf (benchmark.cpp:281-292).  stats (nullable): [1] leaves, [2] triangle tests.

@@ -727,6 +727,7 @@ template <> struct CApi<float> {
     static int device_view(Handle* h, ViewPod* v) { return bvh3f_get_device_view(h, v); }
     static Handle* build(const BBoxPod* b, const VecPod* c, size_t n, const bvh_build_config* cfg) { return bvh3f_build(nullptr, b, c, n, cfg); }
     static Handle* build_triangles(const float* v, size_t n, const bvh_build_config* cfg, unsigned fl) { return bvh3f_build_triangles(v, n, cfg, fl); }
+    static Handle* build_boxes(const BBoxPod* b, const VecPod* c, size_t n, const bvh_build_config* cfg, unsigned fl) { return bvh3f_build_boxes(b, c, n, cfg, fl); }
     static void destroy(Handle* h) { bvh3f_destroy(h); }
     static size_t node_count(Handle* h) { return bvh3f_get_node_count(h); }
     static size_t prim_count(Handle* h) { return bvh3f_get_prim_count(h); }
@@ -740,6 +741,7 @@ template <> struct CApi<double> {
     static int device_view(Handle* h, ViewPod* v) { return bvh3d_get_device_view(h, v); }
     static Handle* build(const BBoxPod* b, const VecPod* c, size_t n, const bvh_build_config* cfg) { return bvh3d_build(nullptr, b, c, n, cfg); }
     static Handle* build_triangles(const double* v, size_t n, const bvh_build_config* cfg, unsigned fl) { return bvh3d_build_triangles(v, n, cfg, fl); }
+    static Handle* build_boxes(const BBoxPod* b, const VecPod* c, size_t n, const bvh_build_config* cfg, unsigned fl) { return bvh3d_build_boxes(b, c, n, cfg, fl); }
     static void destroy(Handle* h) { bvh3d_destroy(h); }
     static size_t node_count(Handle* h) { return bvh3d_get_node_count(h); }
     static size_t prim_count(Handle* h) { return bvh3d_get_prim_count(h); }
@@ -828,6 +830,18 @@ public:
         static_assert(sizeof(Tri<T, 3>) == 9 * sizeof(T));
         handle_ = Api::build_triangles(reinterpret_cast<const T*>(tris.data()), tris.size(), config, 0);
         if (!handle_) throw std::runtime_error(std::string("bvh::v2::cuda::Accel: ") + bvh_last_error());
+    }
+    /// Builds from per-primitive boxes and centres (bvhNN_build_boxes): with flags = BVH_DEVICE_POINTERS both arrays
+    /// are device pointers (on the device of bvh_cuda_set_device), otherwise host pointers.  The same tree as
+    /// DefaultBuilder::build on the same values; reach it from kernels through device_view().
+    static Accel from_boxes(const BBox<T, 3>* bboxes, const Vec<T, 3>* centers, size_t count,
+                            const bvh_build_config* config = nullptr, unsigned flags = 0) {
+        static_assert(sizeof(BBox<T, 3>) == sizeof(typename Api::BBoxPod) && sizeof(Vec<T, 3>) == sizeof(typename Api::VecPod));
+        Accel a;
+        a.handle_ = Api::build_boxes(reinterpret_cast<const typename Api::BBoxPod*>(bboxes),
+                                     reinterpret_cast<const typename Api::VecPod*>(centers), count, config, flags);
+        if (!a.handle_) throw std::runtime_error(std::string("bvh::v2::cuda::Accel::from_boxes: ") + bvh_last_error());
+        return a;
     }
     Accel(Accel&& o) noexcept : handle_(std::exchange(o.handle_, nullptr)) {}
     Accel& operator=(Accel&& o) noexcept { if (this != &o) { reset(); handle_ = std::exchange(o.handle_, nullptr); } return *this; }

@@ -1,11 +1,12 @@
 // include/bvh/v2/cuda/intersect.cuh — traverse a GPU-built BVH from your own CUDA kernels.
 //
-// The reference library has one extension point, Bvh::intersect<IsAnyHit, IsRobust>(ray, start, stack, leaf_fn,
+// The reference library's ray extension point is Bvh::intersect<IsAnyHit, IsRobust>(ray, start, stack, leaf_fn,
 // inner_fn) (reference bvh.h:59-73,159-182): the library walks the tree, the caller intersects the primitives of every
 // leaf it reaches and shrinks ray.tmax on a hit.  DeviceView::intersect is that call on the device, over the tree a
 // handle keeps on its GPU.  It runs the library's own stack machine (bvhb200::traverse_top_down, traverse_core.cuh, the
 // one the batched kernels use), so it visits the same leaves in the same order as the reference's Bvh::intersect on the
-// same tree.
+// same tree.  The general form, Bvh::traverse_top_down with the caller's own node test, is
+// DeviceView::traverse_top_down ("Queries other than rays", below).
 //
 //     bvh3f* bvh = bvh3f_build(nullptr, bboxes, centers, n, nullptr);     // or bvh3f_build_triangles
 //     bvh_device_view3f c;
@@ -40,6 +41,47 @@
 // The inner hook, when given, is called once per inner step with the reference index of the left child of the node
 // being expanded (the right child is that index + 1), before the step's box tests: the reference's InnerFn, which
 // receives those two nodes.
+//
+// Queries other than rays: view.traverse_top_down<IsAnyHit>(start, stack, leaf_fn, node_fn) is the reference's
+// Bvh::traverse_top_down (bvh.h:59-65,124-157), of which intersect is one instance.  It starts at `start`; while the
+// current node is an inner node it calls node_fn on its two children and descends to the near one, pushes the far one
+// when both are hit, and pops the stack when neither is; at a leaf it calls leaf_fn; it ends when the stack is empty.
+//   * node function: called as node_fn(const Node& left, const Node& right) with register copies of the two children
+//     (node.bounds[6] as minx, maxx, miny, maxy, minz, maxz, node.index).  It returns anything that unpacks with a
+//     structured binding into three values convertible to bool, (hit_left, hit_right, should_swap): an aggregate of
+//     three bools, cuda::std::tuple on the device or std::tuple on the host (std::tuple is not device code).
+//     should_swap (visit the right child first) applies when both children are hit, whatever IsAnyHit is;
+//   * leaf function: leaf_fn(size_t begin, size_t end) -> bool with BVH-order slots, as for intersect; with IsAnyHit a
+//     true return ends the traversal.  A leaf `start` gets one leaf_fn call and no node_fn call;
+//   * shared state: the two functions may share state (a search radius the leaf shrinks, a count); every node_fn call
+//     comes after all earlier leaf_fn calls have returned;
+//   * stacks: the same as for intersect, with the same bound, stack_bound() = depth + 1.
+// Each sibling pair is read as one aligned 64-byte (float) / 128-byte (double) block through the read-only path.  A
+// box-overlap query (collision broad phase), counting the primitives whose boxes overlap a query box:
+//
+//     struct Pick { bool left, right, swap; };
+//     __device__ bool overlaps(const float* b, const bvh_bbox3f& q) {        // b: minx, maxx, miny, maxy, minz, maxz
+//         return b[0] <= q.max.x && q.min.x <= b[1] && b[2] <= q.max.y && q.min.y <= b[3] &&
+//                b[4] <= q.max.z && q.min.z <= b[5];
+//     }
+//     __global__ void overlap(View view, const bvh_bbox3f* boxes, const bvh_bbox3f* queries, uint32_t* counts, size_t n) {
+//         const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+//         if (i >= n) return;
+//         const bvh_bbox3f q = queries[i];
+//         View::SmallStack<64> stack;
+//         uint32_t count = 0;
+//         view.traverse_top_down<false>(view.root_index(), stack,
+//             [&](size_t begin, size_t end) {
+//                 for (size_t k = begin; k < end; ++k) {
+//                     const bvh_bbox3f b = boxes[view.prim_id(k)];             // original order
+//                     const float f[6] = { b.min.x, b.max.x, b.min.y, b.max.y, b.min.z, b.max.z };
+//                     count += overlaps(f, q);
+//                 }
+//                 return false;
+//             },
+//             [&](const View::Node& l, const View::Node& r) { return Pick { overlaps(l.bounds, q), overlaps(r.bounds, q), false }; });
+//         counts[i] = count;
+//     }
 //
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
@@ -137,6 +179,16 @@ template <typename T> struct DeviceView {
                 return hit;
             },
             [&](Index first_child) { inner_fn(static_cast<size_t>(first_child)); });
+    }
+
+    // Bvh::traverse_top_down<IsAnyHit> (reference bvh.h:59-65,124-157) with the caller's node test: see "Queries other
+    // than rays" at the top of this file.
+    template <bool IsAnyHit, typename Stack, typename LeafFn, typename NodeFn>
+    BVH_HD void traverse_top_down(Index start, Stack& stack, LeafFn&& leaf_fn, NodeFn&& node_fn) const {
+        bvhb200::traverse_nodes<T, IsAnyHit>(
+            nodes, start, stack,
+            [&](Index begin, Index end) { return static_cast<bool>(leaf_fn(static_cast<size_t>(begin), static_cast<size_t>(end))); },
+            node_fn);
     }
 
     // PrecomputedTri::intersect (reference tri.h:55-74) on BVH-order triangle k: true, with the hit's distance and

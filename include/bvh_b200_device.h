@@ -1,7 +1,8 @@
 /* include/bvh_b200_device.h — C ABI: the device-resident tree of a handle, for CUDA kernels that traverse it with
- * their own leaf functions (include/bvh/v2/cuda/intersect.cuh wraps it for device code), and its refit from
- * per-primitive boxes, so that a tree over primitives of the caller's own (spheres, particles, ...) can follow them as
- * they move without leaving the GPU.  Exported by libbvh_c.so next to the entry points of <bvh_b200.h>.
+ * their own leaf functions (include/bvh/v2/cuda/intersect.cuh wraps it for device code), its build from device-resident
+ * boxes and its refit from per-primitive boxes, so that a tree over primitives of the caller's own (spheres,
+ * particles, ...) can be built and follow them as they move without leaving the GPU.  Exported by libbvh_c.so next to
+ * the entry points of <bvh_b200.h>.
  *
  * struct bvh_device_viewNN — all pointers are device pointers on `device`:
  *   nodes     node_count + 1 records; reference node i (what bvhNN_get_node(bvh, i) shows) is record i + 1,
@@ -58,7 +59,16 @@ extern "C" {
        host pointer the boxes are copied and the call returns when the refit is done.  Non-zero, with a message from     \
        bvh_last_error(), for a NULL handle or bboxes, a prim_count that is not the tree's, or a handle without a tree;    \
        the tree is then left as it was. */                                                                            \
-    BVH_API int bvh##S##_refit_boxes(struct bvh##S* bvh, const struct bvh_bbox##S* bboxes, size_t prim_count, unsigned flags);
+    BVH_API int bvh##S##_refit_boxes(struct bvh##S* bvh, const struct bvh_bbox##S* bboxes, size_t prim_count, unsigned flags); \
+    /* bvhNN_build from boxes and centres that may live on the GPU: with BVH_DEVICE_POINTERS, bboxes and centers are     \
+       device pointers on the device chosen by bvh_cuda_set_device; without it they are host pointers and the call is    \
+       bvhNN_build.  The tree is bit for bit what bvhNN_build gives for the same values and config.  The build runs on  \
+       the new handle's stream (the caller's stream after bvh_cuda_set_stream, otherwise a private one) and the call    \
+       returns after the build's one synchronisation of that stream, so the inputs are no longer read when it returns.  \
+       With a private stream, finish writing the boxes and centres before the call.  NULL, with a message from          \
+       bvh_last_error(), for a NULL bboxes or centers or a prim_count of 0 or beyond the index range. */                  \
+    BVH_API struct bvh##S* bvh##S##_build_boxes(const struct bvh_bbox##S* bboxes, const struct bvh_vec##S* centers,      \
+                                                size_t prim_count, const struct bvh_build_config* config, unsigned flags);
 
 BVH_B200_DECLARE_VIEW(3f)
 BVH_B200_DECLARE_VIEW(3d)
