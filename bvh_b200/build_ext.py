@@ -66,6 +66,8 @@ TEST_KERNELS_SRC = os.path.join(ROOT, "tests", "device_api_kernels.cu")
 TEST_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_api_kernels.so")
 QUERY_KERNELS_SRC = os.path.join(ROOT, "tests", "device_query_kernels.cu")
 QUERY_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_query_kernels.so")
+BOTTOM_UP_KERNELS_SRC = os.path.join(ROOT, "tests", "device_bottom_up_kernels.cu")
+BOTTOM_UP_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_bottom_up_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -102,6 +104,12 @@ def build_device_api_tests(force: bool = False, verbose: bool = False) -> str:
 def build_device_query_tests(force: bool = False, verbose: bool = False) -> str:
     """tests/device_query_kernels.cu: the test kernels of DeviceView::traverse_top_down (box overlap, nearest point)."""
     return _build_test_kernels(QUERY_KERNELS_SRC, QUERY_KERNELS_LIB, force, verbose)
+
+
+def build_device_bottom_up_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_bottom_up_kernels.cu: the test kernels of DeviceView::traverse_bottom_up (counts and boxes, mass and
+    centre, Barnes-Hut through the three-argument node test)."""
+    return _build_test_kernels(BOTTOM_UP_KERNELS_SRC, BOTTOM_UP_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

@@ -15,6 +15,8 @@
 
 #include "core.cuh"
 
+#include <type_traits>
+
 namespace bvhb200 {
 
 // Two adjacent nodes (a sibling pair) in registers.
@@ -253,13 +255,24 @@ BVH_HD void inner_step(const DevNode<T>* __restrict__ nodes, const RayCtx<T>& r,
     descend<U>(l0 <= l1, r0 <= r1, !kAny && l0 > r0, pair.li, pair.ri, top, stack);
 }
 
+// node_fn(left, right, left_index) when it takes the left child's reference index, node_fn(left, right) otherwise.
+template <typename NodeFn, typename Node, typename U>
+BVH_HD decltype(auto) node_test(NodeFn& node_fn, const Node& left, const Node& right, U left_index) {
+    if constexpr (std::is_invocable_v<NodeFn&, const Node&, const Node&, size_t>)
+        return node_fn(left, right, static_cast<size_t>(left_index));
+    else
+        return node_fn(left, right);
+}
+
 // Bvh::traverse_top_down with the caller's node test (reference bvh.h:124-157), for queries other than rays: box
 // overlap, point location, nearest-neighbour searches.  The traversal starts at the node index `start` with an empty
 // stack.
-//   node_fn(const DevNode<T>& left, const DevNode<T>& right)  called once per inner node reached, with register copies
-//                                 of its two children; returns anything that unpacks with a structured binding into
-//                                 (hit_left, hit_right, should_swap), each convertible to bool.  should_swap takes
-//                                 effect when both children are hit, whatever kAny is.
+//   node_fn(const DevNode<T>& left, const DevNode<T>& right[, size_t left_index])  called once per inner node reached,
+//                                 with register copies of its two children and, when it takes a third argument, the
+//                                 reference index of the left child (the right one is left_index + 1); returns anything
+//                                 that unpacks with a structured binding into (hit_left, hit_right, should_swap), each
+//                                 convertible to bool.  should_swap takes effect when both children are hit, whatever
+//                                 kAny is.
 //   leaf_fn(begin, end) -> bool   called on every leaf reached, with its BVH-order primitive range; with kAny a true
 //                                 return ends the traversal.  A leaf `start` is handed to leaf_fn without a node test.
 //   stack                         push(U) and try_pop(U&) (false when empty); it holds at most depth + 1 entries.
@@ -280,8 +293,8 @@ BVH_HD void traverse_nodes(const DevNode<T>* __restrict__ nodes, typename Real<T
             for (int k = 0; k < 6; ++k) { left.bounds[k] = pair.lb[k]; right.bounds[k] = pair.rb[k]; }
             left.index = pair.li; right.index = pair.ri;
             left.pad = right.pad = 0;
-            const auto [hit_left, hit_right, should_swap] = node_fn(static_cast<const DevNode<T>&>(left),
-                                                                    static_cast<const DevNode<T>&>(right));
+            const auto [hit_left, hit_right, should_swap] = node_test(node_fn, static_cast<const DevNode<T>&>(left),
+                                                                      static_cast<const DevNode<T>&>(right), index_first(top));
             descend<U>(static_cast<bool>(hit_left), static_cast<bool>(hit_right), static_cast<bool>(should_swap),
                        pair.li, pair.ri, top, stack);
         }

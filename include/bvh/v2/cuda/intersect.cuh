@@ -47,7 +47,10 @@
 // current node is an inner node it calls node_fn on its two children and descends to the near one, pushes the far one
 // when both are hit, and pops the stack when neither is; at a leaf it calls leaf_fn; it ends when the stack is empty.
 //   * node function: called as node_fn(const Node& left, const Node& right) with register copies of the two children
-//     (node.bounds[6] as minx, maxx, miny, maxy, minz, maxz, node.index).  It returns anything that unpacks with a
+//     (node.bounds[6] as minx, maxx, miny, maxy, minz, maxz, node.index), or as node_fn(left, right, size_t left_index)
+//     when it takes a third argument: the reference index of the left child (the right one is left_index + 1), what
+//     `&left - bvh.nodes.data()` gives on the host, so that it can read data the caller keeps per node (below, "Data per
+//     node").  It returns anything that unpacks with a
 //     structured binding into three values convertible to bool, (hit_left, hit_right, should_swap): an aggregate of
 //     three bools, cuda::std::tuple on the device or std::tuple on the host (std::tuple is not device code).
 //     should_swap (visit the right child first) applies when both children are hit, whatever IsAnyHit is;
@@ -83,6 +86,91 @@
 //         counts[i] = count;
 //     }
 //
+// Data per node: view.traverse_bottom_up(workspace, workspace_bytes, leaf_fn, inner_fn[, stream]) is the reference's
+// Bvh::traverse_bottom_up (bvh.h:184-208), the pass Bvh::refit is built on, for data the caller computes per node: mass
+// and centre of mass (Barnes-Hut), summed power and normal cones (light trees), a subtree's largest radius or speed, its
+// primitive count.  It runs on the GPU, one thread per leaf climbing towards the root, in two kernels on `stream` (the
+// handle's by default) with no host synchronisation: bottom_up_link_kernel, then bottom_up_climb_kernel, over slots
+// [1, node_count].
+//   * leaf_fn(size_t node, size_t begin, size_t end) is called once per leaf, with its reference index and its BVH-order
+//     primitive range [begin, end) (view.prim_id(k) is the original id of slot k, as for intersect);
+//   * inner_fn(size_t node, size_t left) is called once per inner node, with its reference index and its left child's
+//     (the right one is left + 1);
+//   * both are device function objects, copied to the kernel by value: a struct with a __device__ (or
+//     __host__ __device__) operator(), or an extended __device__ lambda (nvcc --extended-lambda);
+//   * every node of a tree whose nodes are all reachable from the root gets exactly one call; every tree the library
+//     builds, and every tree it loads from the reference's format, is such a tree;
+//   * an inner node's call comes after both of its children's calls, and their global writes are visible to it (the
+//     arrival at a parent is an acquire-release atomic at device scope).  Data the pass writes must not be read through
+//     __ldg or a `const __restrict__` pointer inside the pass: the read-only path does not see other threads' writes;
+//   * the order is otherwise unspecified, and differs from run to run on the device.  A function that combines only its
+//     children's values (and its leaf's primitives) therefore gives a result that does not depend on the order;
+//   * workspace: view.bottom_up_workspace_bytes() bytes of device memory, allocated by the caller and not initialised:
+//     the pass writes its parent links and clears its arrival flags itself, so the same workspace serves pass after pass
+//     on one stream.  Two passes must not share one workspace at the same time.  A smaller workspace throws
+//     std::length_error, a failed launch std::runtime_error;
+//   * compiled as plain host C++, the pass runs serially on host-resident copies, in the reference's order: leaves in
+//     descending index, each climbing while both children of the parent are done, which is the call sequence of
+//     Bvh::traverse_bottom_up.
+// Subtree mass and centre of mass, then a Barnes-Hut potential that reads them through the three-argument node test
+// (compile with --fmad=false to match a host computation bit for bit):
+//
+//     struct MassCentre {                                                  // one object serves as leaf_fn and inner_fn
+//         const uint32_t* prim_ids; const float* pos; const float* mass;  // pos: x, y, z per particle, original order
+//         float* node_mass; float* node_centre;                            // node_count and 3 * node_count floats
+//         __device__ void operator()(size_t node, size_t begin, size_t end) const {          // leaf
+//             float m = 0, c[3] = { 0, 0, 0 };
+//             for (size_t k = begin; k < end; ++k) {
+//                 const uint32_t id = prim_ids[k];
+//                 m += mass[id];
+//                 for (int a = 0; a < 3; ++a) c[a] += mass[id] * pos[3 * id + a];
+//             }
+//             node_mass[node] = m;
+//             for (int a = 0; a < 3; ++a) node_centre[3 * node + a] = c[a] / m;
+//         }
+//         __device__ void operator()(size_t node, size_t left) const {                        // inner: after both children
+//             const float ml = node_mass[left], mr = node_mass[left + 1], m = ml + mr;
+//             node_mass[node] = m;
+//             for (int a = 0; a < 3; ++a)
+//                 node_centre[3 * node + a] = (ml * node_centre[3 * left + a] + mr * node_centre[3 * (left + 1) + a]) / m;
+//         }
+//     };
+//     size_t bytes = view.bottom_up_workspace_bytes();                     // on the host
+//     void* workspace; cudaMallocAsync(&workspace, bytes, stream);
+//     const MassCentre mc { view.prim_ids, d_pos, d_mass, d_node_mass, d_node_centre };
+//     view.traverse_bottom_up(workspace, bytes, mc, mc, stream);
+//     potential<<<blocks, 128, 0, stream>>>(view, d_node_mass, d_node_centre, d_pos, d_mass, d_points, m, 0.25f, d_phi);
+//
+//     __global__ void potential(View view, const float* node_mass, const float* node_centre, const float* pos,
+//                               const float* mass, const float* points, size_t m, float theta2, float* phi) {
+//         const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+//         if (i >= m) return;
+//         const float p[3] = { points[3 * i], points[3 * i + 1], points[3 * i + 2] };
+//         auto dist2 = [&](const float* c) { float d = 0; for (int a = 0; a < 3; ++a) d += (c[a] - p[a]) * (c[a] - p[a]); return d; };
+//         float sum = 0;
+//         // far enough (node size < theta * distance): the node's mass at its centre, and no descent
+//         auto open = [&](const View::Node& n, size_t k) {
+//             const float size = fmaxf(fmaxf(n.bounds[1] - n.bounds[0], n.bounds[3] - n.bounds[2]), n.bounds[5] - n.bounds[4]);
+//             const float d2 = dist2(node_centre + 3 * k);
+//             if (size * size < theta2 * d2) { sum -= node_mass[k] / sqrtf(d2); return false; }
+//             return true;
+//         };
+//         View::SmallStack<64> stack;
+//         view.traverse_top_down<false>(view.root_index(), stack,
+//             [&](size_t begin, size_t end) {
+//                 for (size_t k = begin; k < end; ++k) {
+//                     const uint32_t id = view.prim_id(k);
+//                     sum -= mass[id] / sqrtf(dist2(pos + 3 * id));
+//                 }
+//                 return false;
+//             },
+//             [&](const View::Node& l, const View::Node& r, size_t left) {
+//                 const bool open_left = open(l, left), open_right = open(r, left + 1);
+//                 return Pick { open_left, open_right, false };
+//             });
+//         phi[i] = sum;
+//     }
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -98,6 +186,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "refit_core.cuh"
 #include "traverse_core.cuh"
 
 namespace bvh::v2::cuda {
@@ -108,6 +197,22 @@ template <> struct ViewTypes<float>  { using CView = bvh_device_view3f; using Ra
 template <> struct ViewTypes<double> { using CView = bvh_device_view3d; using Ray = bvh_ray3d; };
 struct NoInnerFn { template <typename I> BVH_HD void operator()(I) const {} };
 }
+
+#if defined(__CUDACC__)
+// The two kernels of DeviceView::traverse_bottom_up, one thread per slot of [1, slots).
+template <typename T>
+__global__ void bottom_up_link_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, size_t slots, uint32_t* __restrict__ parent,
+                                      int* __restrict__ flags) {
+    const size_t i = 1 + blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i < slots) bvhb200::refit_link(nodes, slots, i, parent, flags);
+}
+template <typename T, typename LeafFn, typename InnerFn>
+__global__ void bottom_up_climb_kernel(const bvhb200::DevNode<T>* nodes, size_t slots, const uint32_t* __restrict__ parent,
+                                       int* __restrict__ flags, LeafFn leaf_fn, InnerFn inner_fn) {
+    const size_t i = 1 + blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i < slots) bvhb200::climb_from_leaf<T>(nodes, i, parent, flags, leaf_fn, inner_fn);
+}
+#endif
 
 // A plain-data view of one device tree (what bvhNN_get_device_view reports), passed to kernels by value.
 template <typename T> struct DeviceView {
@@ -191,6 +296,52 @@ template <typename T> struct DeviceView {
             node_fn);
     }
 
+    // Bvh::traverse_bottom_up (reference bvh.h:184-208) with the caller's leaf and inner functions: see "Data per node"
+    // at the top of this file.  The workspace is the parent links and the arrival flags, one of each per slot.
+    BVH_HD size_t bottom_up_workspace_bytes() const { return 2 * (node_count + 1) * sizeof(uint32_t); }
+
+    template <typename LeafFn, typename InnerFn>
+    void traverse_bottom_up(void* workspace, size_t workspace_bytes, LeafFn leaf_fn, InnerFn inner_fn) const {
+        traverse_bottom_up(workspace, workspace_bytes, leaf_fn, inner_fn, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <typename LeafFn, typename InnerFn>
+    void traverse_bottom_up(void* workspace, size_t workspace_bytes, LeafFn leaf_fn, InnerFn inner_fn, void* on_stream) const {
+        const size_t need = bottom_up_workspace_bytes();
+        if (workspace_bytes < need || (need && !workspace))
+            throw std::length_error("bvh::v2::cuda::DeviceView::traverse_bottom_up: a workspace of " +
+                                    std::to_string(workspace ? workspace_bytes : 0) + " bytes is too small for " +
+                                    std::to_string(node_count) + " nodes (" + std::to_string(need) + " bytes)");
+        if (node_count == 0) return;
+        const size_t slots = node_count + 1;
+        uint32_t* parent = static_cast<uint32_t*>(workspace);
+        int* flags = reinterpret_cast<int*>(parent + slots);
+#if defined(__CUDACC__)
+        cudaStream_t s = static_cast<cudaStream_t>(on_stream);
+        int previous = 0;
+        check(cudaGetDevice(&previous), "cudaGetDevice");
+        if (previous != device) check(cudaSetDevice(device), "cudaSetDevice");
+        // a slot no inner node points to (possible only in a tree with unreachable nodes) stops the climb
+        cudaError_t e = cudaMemsetAsync(parent, 0, slots * sizeof(uint32_t), s);
+        const unsigned block = 256, grid = (unsigned)((node_count + block - 1) / block);
+        if (e == cudaSuccess) {
+            bottom_up_link_kernel<T><<<grid, block, 0, s>>>(nodes, slots, parent, flags);
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) {
+            bottom_up_climb_kernel<T><<<grid, block, 0, s>>>(nodes, slots, parent, flags, leaf_fn, inner_fn);
+            e = cudaGetLastError();
+        }
+        if (previous != device) cudaSetDevice(previous);
+        check(e, "launch");
+#else
+        (void)on_stream;
+        for (size_t i = 0; i < slots; ++i) parent[i] = 0;
+        for (size_t i = 1; i < slots; ++i) bvhb200::refit_link(nodes, slots, i, parent, flags);
+        for (size_t i = slots; i-- > 1;) bvhb200::climb_from_leaf<T>(nodes, i, parent, flags, leaf_fn, inner_fn);
+#endif
+    }
+
     // PrecomputedTri::intersect (reference tri.h:55-74) on BVH-order triangle k: true, with the hit's distance and
     // barycentrics, when the ray meets it at a distance in [ray.tmin, ray.tmax].  The batched kernels' own test.
     BVH_HD bool intersect_tri(size_t k, const Ray& ray, T& t, T& u, T& v) const {
@@ -205,6 +356,13 @@ template <typename T> struct DeviceView {
     }
 
 private:
+#if defined(__CUDACC__)
+    static void check(cudaError_t e, const char* what) {
+        if (e != cudaSuccess)
+            throw std::runtime_error(std::string("bvh::v2::cuda::DeviceView::traverse_bottom_up: ") + what + ": " +
+                                     cudaGetErrorString(e));
+    }
+#endif
     BVH_HD static void load(const Ray& ray, bvhb200::RayCtx<T>& r) {
         r.org[0] = ray.org.x; r.org[1] = ray.org.y; r.org[2] = ray.org.z;
         r.dir[0] = ray.dir.x; r.dir[1] = ray.dir.y; r.dir[2] = ray.dir.z;
