@@ -68,6 +68,8 @@ QUERY_KERNELS_SRC = os.path.join(ROOT, "tests", "device_query_kernels.cu")
 QUERY_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_query_kernels.so")
 BOTTOM_UP_KERNELS_SRC = os.path.join(ROOT, "tests", "device_bottom_up_kernels.cu")
 BOTTOM_UP_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_bottom_up_kernels.so")
+TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_trace_kernels.cu")
+TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_trace_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -110,6 +112,12 @@ def build_device_bottom_up_tests(force: bool = False, verbose: bool = False) -> 
     """tests/device_bottom_up_kernels.cu: the test kernels of DeviceView::traverse_bottom_up (counts and boxes, mass and
     centre, Barnes-Hut through the three-argument node test)."""
     return _build_test_kernels(BOTTOM_UP_KERNELS_SRC, BOTTOM_UP_KERNELS_LIB, force, verbose)
+
+
+def build_device_trace_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_trace_kernels.cu: the test tracers of DeviceView::trace (triangles, spheres, leaf-call recorders)
+    and the same tracers one thread per ray."""
+    return _build_test_kernels(TRACE_KERNELS_SRC, TRACE_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

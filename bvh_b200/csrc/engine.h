@@ -49,8 +49,8 @@ struct Tunables {
     std::atomic<uint32_t> refill_min { 0 };     // persistent kernels: idle lanes a warp waits for before it draws new rays (1: at once), 0: auto
     std::atomic<uint32_t> wide_budget { 4 };    // same for the wide kernel
     std::atomic<uint32_t> watchdog { 1u << 26 };
-    std::atomic<uint32_t> chunk_rays { 64 };    // persistent kernels: consecutive rays a warp claims at a time (its cohorts are drawn from them)
-    std::atomic<int> stack_round { 2 };         // traversal stack entries are rounded up to a multiple of this (A/B: 8)
+    std::atomic<uint32_t> chunk_rays { kDefaultRunRays };    // persistent kernels: consecutive rays a warp claims at a time (its cohorts are drawn from them)
+    std::atomic<int> stack_round { (int)kDefaultStackRound };         // traversal stack entries are rounded up to a multiple of this (A/B: 8)
     std::atomic<int> smem_carveout { -1 };      // persistent kernels: preferred shared-memory carve-out in percent, -1: the driver's choice
     std::atomic<int> treelet_blocks { 3 };      // treelet kernel: resident blocks per SM its registers are limited for (2 / 3 / 4)
     std::atomic<int> sort_onesweep { 1 };       // build: 1 one-sweep radix sort (one kernel per pass), 0 histogram / scan / scatter per pass

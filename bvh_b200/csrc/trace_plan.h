@@ -74,4 +74,37 @@ inline TracePlan plan_trace(const TraceRequest& q) {
     return p;
 }
 
+// The default length of a persistent warp's private run of consecutive rays (Tunables::chunk_rays, the switch
+// "chunk_rays"), and the default rounding of the traversal stack's entries (Tunables::stack_round).
+constexpr uint32_t kDefaultRunRays = 64;
+constexpr uint32_t kDefaultStackRound = 2;
+
+// The run a persistent warp claims with one global atomic: `chunk_rays` at most, and shorter for small batches, so that
+// every resident warp gets about 8 runs (tail balance), in multiples of 32 rays and never fewer than 32.
+inline uint32_t persistent_run_rays(uint32_t chunk_rays, unsigned long long n, int sm_count) {
+    uint32_t run = chunk_rays;
+    const unsigned long long fair = n / ((unsigned long long)sm_count * 32ull * 8ull);
+    if (fair < run) run = (uint32_t)fair;
+    run &= ~31u;
+    return run < 32u ? 32u : run;
+}
+
+// The grid of a persistent launch: one resident wave (SM count x resident blocks per SM, at least one), never more
+// blocks than the batch can feed at `rays_per_warp` rays per warp.
+inline unsigned long long persistent_grid(int sm_count, int blocks_per_sm, unsigned long long n, unsigned rays_per_warp,
+                                          unsigned warps_per_block) {
+    if (blocks_per_sm < 1) blocks_per_sm = 1;
+    unsigned long long grid = (unsigned long long)sm_count * blocks_per_sm;
+    const unsigned long long max_useful = (n + rays_per_warp - 1) / rays_per_warp / warps_per_block + 1;
+    return grid > max_useful ? max_useful : grid;
+}
+
+// Shared-memory stack entries per thread of a tree of `depth`: depth + 1 pending far children at most and the sentinel,
+// rounded up to a multiple of `round`, and at least 16.
+inline uint32_t stack_entries(uint32_t depth, uint32_t round) {
+    uint32_t entries = depth + 2;
+    entries = (entries + round - 1u) / round * round;
+    return entries < 16 ? 16 : entries;
+}
+
 } // namespace bvhb200

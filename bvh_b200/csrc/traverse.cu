@@ -28,6 +28,7 @@
 
 #include "build_core.cuh"
 #include "engine.h"
+#include "persistent_core.cuh"
 #include "radix_sort.cuh"
 #include "traverse_core.cuh"
 #include "wide_bvh.cuh"
@@ -36,14 +37,7 @@ namespace bvhb200 {
 
 namespace {
 
-// Resident blocks per SM the persistent kernel's registers are limited for (float, the variants without hit staging):
-// 8 -> 64 registers, 9 -> 56, 10 -> 48.  The kernel is latency-bound, so more resident warps per SM hide more of it; on
-// the H100 (bench.py c2 / c3) 12 blocks (40 registers, spills) were measured 1.4x slower than 9.  The variants with
-// warp-staged hit stores (kGather) keep 8.
-#ifndef BVH_TRACE_BLOCKS
-#define BVH_TRACE_BLOCKS 9
-#endif
-constexpr int kTraceBlock = 128;
+// (kTraceBlock, BVH_TRACE_BLOCKS and the persistent kernels' warp scheduler: persistent_core.cuh)
 constexpr uint32_t kPairRunRays = 128;   // the lane-pair kernel's runs: fixed, the chunk_rays switch does not apply to it
 
 // One ray record into registers.  kStreamed: from global memory, read once (ld.global.cs, evict-first); otherwise a plain
@@ -348,32 +342,8 @@ __device__ __forceinline__ void retire_ray(HitStager<T>& st, const HitSinks<T>& 
 }
 
 // ---- the ray feed of the persistent kernels ------------------------------------------------------------------
-// A warp claims private runs of consecutive batch positions with one global atomicAdd per run and hands them to its idle
-// lanes by ballot + prefix rank (active-mask compaction).  A warp draws new rays only once refill_min of its lanes are
-// idle: the rays drawn together are neighbours (consecutive positions of one run) and start at the root in the same
-// iteration, so they stay in step through the top of the tree and their node fetches — same address in the same
-// instruction — cost one L1 wavefront instead of one per lane; the price is idle lanes, which these L1-bound kernels can
-// afford.
-
-// A round past the watchdog's limit sets the status word: a hang becomes an error (see trace_rays).
-__device__ __forceinline__ bool watchdog_fired(uint32_t& rounds, uint32_t limit, uint32_t* status, unsigned lane) {
-    if (++rounds <= limit) return false;
-    if (lane == 0) atomicExch(status, 1u);
-    return true;
-}
-
-// First position of a new run of `run` positions (warp-uniform; it may lie beyond the batch).
-__device__ __forceinline__ unsigned long long claim_run(unsigned long long* next_ray, uint32_t run, unsigned lane, unsigned mask) {
-    unsigned long long first = 0;
-    if (lane == 0) first = atomicAdd(next_ray, (unsigned long long)run);
-    return __shfl_sync(mask, first, 0);
-}
-
-// The rest of the warp's current run, and whether the batch has no rays left (warp-uniform).
-struct RunCursor {
-    unsigned long long pos = 0, end = 0;
-    bool exhausted = false;
-};
+// (the scheduler — claim_run, RunCursor, refill_lanes, run_rounds — is persistent_core.cuh's; the draws below add the
+// TMA staging, the gather mode's staging groups and the ray reordering of the library's triangle kernels)
 
 // One draw: the lanes of `idle` (`rank`: this lane's rank among them) take the next popc(idle) positions of the run at
 // most, clipped to the batch and, in gather mode, to the staging group of 32 consecutive rays the run is in.  Claims a new
@@ -419,58 +389,23 @@ __device__ __forceinline__ bool start_ray(const RayCtx<T>& r, HitState<T>& hit, 
     return true;
 }
 
-// Refills the warp's idle lanes among `lanes`, once refill_min of them are idle, until none is idle or the batch has no
-// rays left.  draw(idle, rank) hands out one round of rays (rank: the lane's rank in `idle`, counted over lt_mask); it
-// returns false when the batch has none left.
-template <typename T, bool kGather, typename Draw>
-__device__ __forceinline__ void refill_lanes(const bool& has_ray, const RunCursor& c, unsigned lanes, uint32_t refill_min,
-                                             unsigned lt_mask, unsigned mask, HitStager<T>& stager, const HitSinks<T>& sinks,
-                                             unsigned lane, Draw&& draw) {
-    unsigned idle = __ballot_sync(mask, !has_ray) & lanes;
-    if ((uint32_t)__popc(idle) < refill_min) idle = 0u;
-    while (idle != 0u && !c.exhausted) {
-        if (!draw(idle, (unsigned)__popc(idle & lt_mask))) break;
-        if (kGather) stager_account(stager, sinks, lane);      // (a NaN ray may just have been retired)
-        idle = __ballot_sync(mask, !has_ray) & lanes;
-    }
-}
-
 constexpr int kTmaChunkRays = 32;        // rays per bulk copy (1 KB of float rays), two buffers per warp
 
 template <typename T> __host__ __device__ constexpr size_t tma_smem_bytes() {
     return (size_t)(kTraceBlock / 32) * 2 * kTmaChunkRays * sizeof(DevRay<T>) + (size_t)(kTraceBlock / 32) * 2 * 8;
 }
 
-// The rounds of a persistent kernel, until the batch has no rays left.  A round: the watchdog (`rounds`: the count to
-// start from); refill_lanes through draw(idle, rank); the kernel's inner phase inner(), which retires the rays it
-// finishes; the leaf phase, which retires a ray on an any-hit hit or an empty stack.  `mask` is the member mask of every
-// warp primitive.  The lane's ray state (has_ray, top, r, hit, stack) belongs to the kernel; retire() stores its record.
-template <typename T, bool kAny, bool kGather, typename U, typename Stack, typename Draw, typename Retire, typename Inner>
-__device__ __forceinline__ void run_rounds(const TraceArgs<T>& a, const RunCursor& run, bool& has_ray, U& top, RayCtx<T>& r,
-                                           HitState<T>& hit, Stack& stack, HitStager<T>& stager, unsigned mask, uint32_t rounds,
-                                           unsigned lanes, uint32_t refill_min, unsigned lt_mask, bool lowest_id, unsigned lane,
-                                           Draw&& draw, Retire&& retire, Inner&& inner) {
-    for (;;) {
-        if (watchdog_fired(rounds, a.watchdog, a.status, lane)) return;
-        refill_lanes<T, kGather>(has_ray, run, lanes, refill_min, lt_mask, mask, stager, a.hits, lane, draw);
-        if (__ballot_sync(mask, has_ray) == 0u) {
-            if (run.exhausted) break;                        // nothing in flight and nothing left
-            continue;                                        // (only NaN rays were drawn: refill again)
+// The leaf phase of the triangle kernels: the lane's leaf, then its ray retires on an any-hit hit or an empty stack.
+template <typename T, bool kAny, typename U, typename Stack, typename Retire>
+__device__ __forceinline__ void triangle_leaf_phase(const TraceArgs<T>& a, bool lowest_id, bool& has_ray, U& top, RayCtx<T>& r,
+                                                    HitState<T>& hit, Stack& stack, Retire&& retire) {
+    if (has_ray && index_count(top) != 0) {
+        leaf_step<T>(a.tris, a.prim_ids, lowest_id, top, r, hit, nullptr);
+        if ((kAny && hit.slot != kInvalidId) || !stack.try_pop(top)) {
+            retire();
+            has_ray = false;
         }
-        inner();
-        __syncwarp(mask);
-
-        if (has_ray && index_count(top) != 0) {
-            leaf_step<T>(a.tris, a.prim_ids, lowest_id, top, r, hit, nullptr);
-            if ((kAny && hit.slot != kInvalidId) || !stack.try_pop(top)) {
-                retire();
-                has_ray = false;
-            }
-        }
-        __syncwarp(mask);
-        if (kGather) stager_account(stager, a.hits, lane);
     }
-    if (kGather && stager.buf && lane == 0) bulk_wait_all();         // the last bulk stores have left shared memory and landed
 }
 
 // Persistent kernel.  kTma = true stages the warp's next ray chunk into shared memory with a bulk
@@ -595,8 +530,11 @@ trace_persistent_kernel(TraceArgs<T> a) {
             }
         }
     };
-    run_rounds<T, kAny, kGather>(a, run, has_ray, top, r, hit, stack, stager, kFull, 0u, kFull, a.refill_min, lt_mask, lowest_id,
-                                 lane, draw, retire, inner);
+    auto account = [&] { if (kGather) stager_account(stager, a.hits, lane); };
+    auto leaf = [&] { triangle_leaf_phase<T, kAny>(a, lowest_id, has_ray, top, r, hit, stack, retire); };
+    // (finish: the last bulk stores have left shared memory and landed)
+    auto finish = [&] { if (kGather && stager.buf && lane == 0) bulk_wait_all(); };
+    run_rounds<true>(run, has_ray, kFull, 0u, a.watchdog, a.status, kFull, a.refill_min, lt_mask, lane, draw, account, inner, leaf, finish);
 }
 
 // ---- lane-pair kernel ------------------------------------------------------------------------------
@@ -666,7 +604,7 @@ trace_pair_kernel(TraceArgs<T> a) {
     uint32_t rounds = lane_zero;
     for (;;) {
         if (watchdog_fired(rounds, a.watchdog, a.status, lane)) return;
-        refill_lanes<T, false>(has_ray, run, kEven, 0u, lt_mask, kFull, stager, a.hits, lane, draw);
+        refill_lanes(has_ray, run, kEven, 0u, lt_mask, kFull, draw, [] {});
         if (__ballot_sync(kFull, has_ray) == 0u) {
             if (run.exhausted) break;
             continue;
@@ -791,8 +729,11 @@ trace_wide_kernel(TraceArgs<float> a) {
         }
     };
     // (plan_trace never chooses this kernel for BVH_TIE_LAST_VISITED: the lowest id wins ties)
-    run_rounds<float, kAny, kGather>(a, run, has_ray, top, r, hit, stack, stager, kFull, 0u, kFull, a.refill_min, lt_mask, true, lane,
-                                     draw, retire, inner);
+    auto account = [&] { if (kGather) stager_account(stager, a.hits, lane); };
+    auto leaf = [&] { triangle_leaf_phase<float, kAny>(a, true, has_ray, top, r, hit, stack, retire); };
+    // (finish: the last bulk stores have left shared memory and landed)
+    auto finish = [&] { if (kGather && stager.buf && lane == 0) bulk_wait_all(); };
+    run_rounds<true>(run, has_ray, kFull, 0u, a.watchdog, a.status, kFull, a.refill_min, lt_mask, lane, draw, account, inner, leaf, finish);
 }
 
 
@@ -880,10 +821,7 @@ int launch_persistent(KernelT kernel, const TraceArgs<T>& args, size_t smem, uns
     int sm_count = 132, per_sm = 1;
     BVH_CUDA_TRY(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device));
     BVH_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kTraceBlock, smem));
-    if (per_sm < 1) per_sm = 1;
-    unsigned long long grid = (unsigned long long)sm_count * per_sm;
-    const unsigned long long max_useful = (args.n + rays_per_warp - 1) / rays_per_warp / (kTraceBlock / 32) + 1;
-    if (grid > max_useful) grid = max_useful;
+    const unsigned long long grid = persistent_grid(sm_count, per_sm, args.n, rays_per_warp, kTraceBlock / 32);
     BVH_CUDA_TRY(cudaMemsetAsync(args.next_ray, 0, sizeof(unsigned long long), stream));
     kernel<<<(unsigned)grid, kTraceBlock, smem, stream>>>(args);
     return 0;
@@ -973,13 +911,8 @@ int trace_rays(const DeviceBvh<T>& bvh, const DevRay<T>* d_rays, DevHit<T>* d_hi
     bvh.last_kernel = plan.kernel;
     args.ray_stats = d_ray_stats;
     args.lowest_id = (flags & kTraceLastVisited) ? 0 : 1;
-    uint32_t entries = bvh.depth + 2;                           // depth + 1 pending far children at most, + the sentinel
-    {                                                           // (an entry is one 512-byte row of the block: any count keeps the alignment)
-        const uint32_t r = (uint32_t)tun.stack_round.load();
-        entries = (entries + r - 1u) / r * r;
-    }
-    if (entries < 16) entries = 16;
-    args.stack_entries = entries;
+    // (an entry is one 512-byte row of the block: any count keeps the alignment)
+    args.stack_entries = stack_entries(bvh.depth, (uint32_t)tun.stack_round.load());
     args.wide = nullptr; args.wide_entries = 0;
     if (plan.kernel == kKernelWide) {
         args.wide = bvh.wide;
@@ -988,14 +921,10 @@ int trace_rays(const DeviceBvh<T>& bvh, const DevRay<T>* d_rays, DevHit<T>* d_hi
     }
     args.inner_budget = plan.inner_budget;
     args.refill_min = plan.refill_min;
-    {   // a warp's private run of consecutive rays: as long as the batch allows with ~8 runs per resident warp (tail balance)
-        uint32_t run = tun.chunk_rays.load();
+    {   // a warp's private run of consecutive rays
         int sm_count = 132;
         BVH_CUDA_TRY(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, bvh.device));
-        const unsigned long long fair = n / ((unsigned long long)sm_count * 32ull * 8ull);
-        if (fair < run) run = (uint32_t)fair;
-        run &= ~31u;
-        args.chunk_rays = run < 32u ? 32u : run;
+        args.chunk_rays = persistent_run_rays(tun.chunk_rays.load(), n, sm_count);
     }
     args.watchdog = tun.watchdog.load();
     args.full_mask = 0xFFFFFFFFu;

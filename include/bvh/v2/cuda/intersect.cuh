@@ -171,6 +171,54 @@
 //         phi[i] = sum;
 //     }
 //
+// Whole batches: view.trace<IsAnyHit, IsRobust>(n, tracer, workspace, workspace_bytes[, stream]) traces rays 0 .. n-1
+// with the library's persistent scheduler, the one bvhNN_intersect_rays uses (persistent_core.cuh): persistent warps,
+// runs of consecutive rays claimed with one atomic, idle lanes refilled together once enough of them are idle, a
+// bounded inner phase and one leaf per round, a shared-memory stack.  Neighbouring rays start together and share their
+// node fetches, which one thread per ray through intersect does not get.  The tracer is a plain struct copied to the
+// kernel by value, with a Payload type (per-ray state, kept in registers) and three __device__ (or __host__ __device__)
+// functions:
+//     Ray  start(size_t i, Payload& p) const;                              // ray i of the batch; sets up p
+//     bool leaf(Payload& p, Ray& ray, size_t begin, size_t end) const;    // intersect's leaf_fn
+//     void finish(size_t i, const Payload& p, const Ray& ray) const;      // ray i is done
+//   * for every i in [0, n), start is called once, then the leaf calls, then finish once.  The leaf calls of a ray are
+//     exactly those intersect<IsAnyHit, IsRobust>(ray, root_index(), stack, leaf) makes on the same tree: the same
+//     (begin, end) ranges in the same order.  A ray whose interval is a NaN at the start gets no leaf call when the root
+//     is an inner node and one when it is a leaf; after a leaf that makes the interval a NaN, the remaining stack
+//     entries are drawn without box tests, as traverse_top_down does;
+//   * leaf may change ray.tmin and ray.tmax, and the next box test reads them; other ray fields are read once, from
+//     what start returned.  With IsAnyHit a true return ends the ray.  finish receives the ray with its final interval;
+//   * rays are drawn in index order, in runs per warp, so neighbouring indices share node fetches: number the rays
+//     coherently (by pixel tile, by origin) to get coherence.  No ordering holds between different rays;
+//   * the three functions run on a subset of a warp's lanes: they must not use __syncthreads or full-mask warp
+//     collectives;
+//   * there is no watchdog (intersect has none either): a leaf function that never returns hangs the kernel;
+//   * the call is stream-ordered on `stream` (the handle's by default), does not synchronise the host, and sets and
+//     restores the current device.  n == 0 launches nothing.  Scheduling uses the library's defaults for a
+//     closest-hit or any-hit batch (plan_trace, trace_plan.h); there is nothing to set;
+//   * workspace: view.trace_workspace_bytes() bytes of device memory (the run cursor), allocated by the caller and not
+//     initialised: trace resets it on the stream.  Two calls must not share a workspace at the same time.  A smaller
+//     workspace throws std::length_error, and so does a tree whose shared-memory stack would exceed the 200 KB a
+//     persistent block may have (float: depth > 398); a failed launch throws std::runtime_error;
+//   * compiled as plain host C++, trace runs the rays serially: start, intersect with a host stack of stack_bound()
+//     entries, finish.
+// The kernel is bvh::v2::cuda::device_view_trace_kernel<T, IsAnyHit, IsRobust, Tracer>, 128 threads per block; its
+// registers are limited for 9 resident blocks per SM (float) or 4 (double), as the library's persistent kernel's are, so
+// a payload of more than a few words spills.  A sphere tracer (INTEGRATION.md §5 has it whole):
+//
+//     struct SphereTracer {
+//         struct Payload { uint32_t best; };
+//         const bvh_ray3f* rays; const float4* spheres; const uint32_t* prim_ids; uint32_t* hit_ids;
+//         __device__ bvh_ray3f start(size_t i, Payload& p) const { p.best = UINT32_MAX; return rays[i]; }
+//         __device__ bool leaf(Payload& p, bvh_ray3f& ray, size_t begin, size_t end) const {
+//             for (size_t k = begin; k < end; ++k)
+//                 if (float t; hit_sphere(spheres[prim_ids[k]], ray, t)) { ray.tmax = t; p.best = prim_ids[k]; }
+//             return p.best != UINT32_MAX;
+//         }
+//         __device__ void finish(size_t i, const Payload& p, const bvh_ray3f&) const { hit_ids[i] = p.best; }
+//     };
+//     view.trace<false, false>(n, SphereTracer { d_rays, d_spheres, view.prim_ids, d_hit_ids }, workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -185,8 +233,11 @@
 #include <cstdint>
 #include <stdexcept>
 #include <string>
+#include <vector>
 
+#include "persistent_core.cuh"
 #include "refit_core.cuh"
+#include "trace_plan.h"
 #include "traverse_core.cuh"
 
 namespace bvh::v2::cuda {
@@ -196,6 +247,29 @@ template <typename T> struct ViewTypes;
 template <> struct ViewTypes<float>  { using CView = bvh_device_view3f; using Ray = bvh_ray3f; };
 template <> struct ViewTypes<double> { using CView = bvh_device_view3d; using Ray = bvh_ray3d; };
 struct NoInnerFn { template <typename I> BVH_HD void operator()(I) const {} };
+template <typename T, typename Ray> BVH_HD void load_ray(const Ray& ray, bvhb200::RayCtx<T>& r) {
+    r.org[0] = ray.org.x; r.org[1] = ray.org.y; r.org[2] = ray.org.z;
+    r.dir[0] = ray.dir.x; r.dir[1] = ray.dir.y; r.dir[2] = ray.dir.z;
+    r.tmin = ray.tmin; r.tmax = ray.tmax;
+}
+template <typename Ray, typename T> BVH_HD Ray make_ray(const bvhb200::RayCtx<T>& r) {
+    Ray ray;
+    ray.org.x = r.org[0]; ray.org.y = r.org[1]; ray.org.z = r.org[2];
+    ray.dir.x = r.dir[0]; ray.dir.y = r.dir[1]; ray.dir.z = r.dir[2];
+    ray.tmin = r.tmin; ray.tmax = r.tmax;
+    return ray;
+}
+// DeviceView::trace's stack when the header is compiled as host C++
+template <typename U> struct VectorStack {
+    std::vector<U> elems;
+    void push(U v) { elems.push_back(v); }
+    bool try_pop(U& out) {
+        if (elems.empty()) return false;
+        out = elems.back();
+        elems.pop_back();
+        return true;
+    }
+};
 }
 
 #if defined(__CUDACC__)
@@ -211,6 +285,86 @@ __global__ void bottom_up_climb_kernel(const bvhb200::DevNode<T>* nodes, size_t 
                                        int* __restrict__ flags, LeafFn leaf_fn, InnerFn inner_fn) {
     const size_t i = 1 + blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i < slots) bvhb200::climb_from_leaf<T>(nodes, i, parent, flags, leaf_fn, inner_fn);
+}
+
+// The kernel of DeviceView::trace: the library's persistent scheduler (persistent_core.cuh) over the caller's tracer.
+// Each warp claims runs of `run_rays` consecutive ray indices from `cursor`; a lane draws ray i through
+// tracer.start, descends with the library's inner step (a lane whose interval is a NaN pops its stack instead, as
+// bvhb200::traverse_top_down does), hands its leaf to tracer.leaf and retires the ray through tracer.finish.
+template <typename T, bool IsAnyHit, bool IsRobust, typename Tracer>
+__global__ void __launch_bounds__(bvhb200::kTraceBlock, sizeof(T) == 4 ? BVH_TRACE_BLOCKS : 4)
+device_view_trace_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned long long n, unsigned long long* cursor,
+                         uint32_t run_rays, uint32_t refill_min, uint32_t inner_budget, Tracer tracer) {
+    using U = typename bvhb200::Real<T>::UInt;
+    using Ray = typename detail::ViewTypes<T>::Ray;
+    extern __shared__ __align__(128) unsigned char device_view_trace_smem[];
+    constexpr unsigned kFull = 0xFFFFFFFFu;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    bvhb200::SmemStack<U> stack { reinterpret_cast<U*>(device_view_trace_smem) + threadIdx.x, bvhb200::kTraceBlock, 0 };
+    const U root_index = nodes[1].index;
+
+    bvhb200::RunCursor run;
+    bool has_ray = false;
+    unsigned long long index = 0;
+    bvhb200::RayCtx<T> r;
+    typename Tracer::Payload payload;
+    U top = 0;
+    auto retire = [&] {
+        tracer.finish(static_cast<size_t>(index), static_cast<const typename Tracer::Payload&>(payload), detail::make_ray<Ray>(r));
+        has_ray = false;
+    };
+
+    // one draw: the idle lanes take the next rays of the warp's run, claiming a new run when it is used up
+    auto draw = [&] (unsigned idle, unsigned rank) {
+        if (run.pos == run.end) {
+            const unsigned long long first = bvhb200::claim_run(cursor, run_rays, lane, kFull);
+            if (first >= n) { run.exhausted = true; return false; }
+            run.pos = first;
+            run.end = first + run_rays < n ? first + run_rays : n;
+        }
+        const unsigned avail = (unsigned)(run.end - run.pos), want = __popc(idle);
+        const unsigned take = want < avail ? want : avail;
+        if (!has_ray && rank < take) {
+            index = run.pos + rank;
+            detail::load_ray<T>(tracer.start(static_cast<size_t>(index), payload), r);
+            bvhb200::ray_prologue<T, IsRobust>(r);
+            top = root_index;
+            stack.clear();
+            has_ray = true;
+        }
+        run.pos += take;
+        return true;
+    };
+
+    // inner phase: descend until this lane holds a leaf, its ray is finished, or the step budget of this round is spent
+    auto inner = [&] {
+        if (has_ray) {
+            uint32_t budget = inner_budget;
+            const bool nan = bvhb200::ray_interval_is_nan(r);
+            while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone ends it too)
+                --budget;
+                if (nan) top = bvhb200::pop_or_done<U>(stack);           // both children missed, no box test
+                else bvhb200::inner_step<T, IsAnyHit, IsRobust>(nodes, r, top, stack);
+            }
+            if (top == bvhb200::kTraversalDone<U>) retire();
+        }
+    };
+
+    // leaf phase: the caller's leaf, whose interval the next box test reads; the ray ends on an any-hit hit or an empty stack
+    auto leaf = [&] {
+        if (has_ray && bvhb200::index_count(top) != 0) {
+            const U first = bvhb200::index_first(top);
+            Ray ray = detail::make_ray<Ray>(r);
+            const bool hit = static_cast<bool>(tracer.leaf(payload, ray, static_cast<size_t>(first),
+                                                           static_cast<size_t>(first + (U)bvhb200::index_count(top))));
+            r.tmin = ray.tmin;
+            r.tmax = ray.tmax;
+            if ((IsAnyHit && hit) || !stack.try_pop(top)) retire();
+        }
+    };
+    bvhb200::run_rounds<false>(run, has_ray, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
+                               [] {});
 }
 #endif
 
@@ -342,6 +496,79 @@ template <typename T> struct DeviceView {
 #endif
     }
 
+    // A whole batch of rays on the library's persistent scheduler, with the caller's per-ray functions: see "Whole
+    // batches" at the top of this file.  The workspace is the warps' run cursor.
+    BVH_HD size_t trace_workspace_bytes() const { return sizeof(unsigned long long); }
+
+    template <bool IsAnyHit, bool IsRobust, typename Tracer>
+    void trace(size_t n, const Tracer& tracer, void* workspace, size_t workspace_bytes) const {
+        trace<IsAnyHit, IsRobust>(n, tracer, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsAnyHit, bool IsRobust, typename Tracer>
+    void trace(size_t n, const Tracer& tracer, void* workspace, size_t workspace_bytes, void* on_stream) const {
+        const size_t need = trace_workspace_bytes();
+        if (workspace_bytes < need || !workspace)
+            throw std::length_error("bvh::v2::cuda::DeviceView::trace: a workspace of " + std::to_string(workspace ? workspace_bytes : 0) +
+                                    " bytes is too small (" + std::to_string(need) + " bytes)");
+        // the batched kernels' shared-memory stack, sized and bounded as bvhNN_intersect_rays sizes and bounds it
+        const size_t smem = (size_t)bvhb200::stack_entries(static_cast<uint32_t>(depth), bvhb200::kDefaultStackRound) *
+                            bvhb200::kTraceBlock * sizeof(Index);
+        if (smem > kMaxTraceSmem)
+            throw std::length_error("bvh::v2::cuda::DeviceView::trace: a tree of depth " + std::to_string(depth) + " needs " +
+                                    std::to_string(smem) + " bytes of shared-memory stack per block, more than " +
+                                    std::to_string(kMaxTraceSmem));
+        if (n == 0) return;
+#if defined(__CUDACC__)
+        cudaStream_t s = static_cast<cudaStream_t>(on_stream);
+        int previous = 0;
+        check(cudaGetDevice(&previous), "cudaGetDevice", "trace");
+        if (previous != device) check(cudaSetDevice(device), "cudaSetDevice", "trace");
+        void (*kernel)(const Node*, unsigned long long, unsigned long long*, uint32_t, uint32_t, uint32_t, Tracer) =
+            device_view_trace_kernel<T, IsAnyHit, IsRobust, Tracer>;
+        int sm_count = 0, per_sm = 0;
+        cudaError_t e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device);
+        if (e == cudaSuccess && smem > 48 * 1024) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, bvhb200::kTraceBlock, smem);
+        if (e == cudaSuccess) e = cudaMemsetAsync(workspace, 0, need, s);
+        if (e == cudaSuccess) {
+            // the library's scheduling of a persistent closest-hit or any-hit batch, with its default settings
+            bvhb200::TraceRequest request {};
+            request.flags = bvhb200::kTraceNoTma | (IsAnyHit ? bvhb200::kTraceAnyHit : 0u) | (IsRobust ? bvhb200::kTraceRobust : 0u);
+            request.is_float = sizeof(T) == 4;
+            request.n = n;
+            const bvhb200::TracePlan plan = bvhb200::plan_trace(request);
+            const uint32_t run_rays = bvhb200::persistent_run_rays(bvhb200::kDefaultRunRays, n, sm_count);
+            const unsigned long long grid = bvhb200::persistent_grid(sm_count, per_sm, n, 32, bvhb200::kTraceBlock / 32);
+            kernel<<<(unsigned)grid, bvhb200::kTraceBlock, smem, s>>>(nodes, n, static_cast<unsigned long long*>(workspace), run_rays,
+                                                                     plan.refill_min, plan.inner_budget, tracer);
+            e = cudaGetLastError();
+        }
+        if (previous != device) cudaSetDevice(previous);
+        check(e, "launch", "trace");
+#else
+        (void)on_stream;
+        using Payload = typename Tracer::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            const Ray start = tracer.start(i, payload);
+            Ray ray = start;
+            detail::VectorStack<Index> stack;
+            stack.elems.reserve(stack_bound());
+            intersect<IsAnyHit, IsRobust>(ray, root_index(), stack, [&](size_t begin, size_t end) {
+                Ray leaf_ray = start;                        // (other fields are read once, as on the device)
+                leaf_ray.tmin = ray.tmin; leaf_ray.tmax = ray.tmax;
+                const bool hit = static_cast<bool>(tracer.leaf(payload, leaf_ray, begin, end));
+                ray.tmin = leaf_ray.tmin; ray.tmax = leaf_ray.tmax;
+                return hit;
+            });
+            Ray out = start;
+            out.tmin = ray.tmin; out.tmax = ray.tmax;
+            tracer.finish(i, static_cast<const Payload&>(payload), out);
+        }
+#endif
+    }
+
     // PrecomputedTri::intersect (reference tri.h:55-74) on BVH-order triangle k: true, with the hit's distance and
     // barycentrics, when the ray meets it at a distance in [ray.tmin, ray.tmax].  The batched kernels' own test.
     BVH_HD bool intersect_tri(size_t k, const Ray& ray, T& t, T& u, T& v) const {
@@ -356,18 +583,15 @@ template <typename T> struct DeviceView {
     }
 
 private:
+    // the shared memory a persistent block may have, as bvhNN_intersect_rays bounds it
+    static constexpr size_t kMaxTraceSmem = 200 * 1024;
 #if defined(__CUDACC__)
-    static void check(cudaError_t e, const char* what) {
+    static void check(cudaError_t e, const char* what, const char* call = "traverse_bottom_up") {
         if (e != cudaSuccess)
-            throw std::runtime_error(std::string("bvh::v2::cuda::DeviceView::traverse_bottom_up: ") + what + ": " +
-                                     cudaGetErrorString(e));
+            throw std::runtime_error(std::string("bvh::v2::cuda::DeviceView::") + call + ": " + what + ": " + cudaGetErrorString(e));
     }
 #endif
-    BVH_HD static void load(const Ray& ray, bvhb200::RayCtx<T>& r) {
-        r.org[0] = ray.org.x; r.org[1] = ray.org.y; r.org[2] = ray.org.z;
-        r.dir[0] = ray.dir.x; r.dir[1] = ray.dir.y; r.dir[2] = ray.dir.z;
-        r.tmin = ray.tmin; r.tmax = ray.tmax;
-    }
+    BVH_HD static void load(const Ray& ray, bvhb200::RayCtx<T>& r) { detail::load_ray<T>(ray, r); }
 };
 
 } // namespace bvh::v2::cuda
