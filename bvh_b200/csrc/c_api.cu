@@ -131,9 +131,18 @@ struct DeviceGuard {
 };
 #define BVH_ON_DEVICE(device) DeviceGuard device_guard__(device); if (!device_guard__.ok) return -1
 
-// ---- host mirror ------------------------------------------------------------------------------
-template <typename T> struct HostNode { T bounds[6]; typename Real<T>::UInt index; };
-static_assert(sizeof(HostNode<float>) == 28 && sizeof(HostNode<double>) == 56, "reference Node<T,3> layout");
+// ---- host trees -------------------------------------------------------------------------------
+// The reference's Node<T, kDim> (bounds as min0 max0 min1 max1 ..., then the packed index; node.h:31-37) and the
+// node and primitive-id vectors of its Bvh (bvh.h:17-23).  A 2-D handle is a HostTree; a 3-D handle holds one as
+// its mirror.
+template <typename T, int kDim> struct HostNode { T bounds[2 * kDim]; typename Real<T>::UInt index; };
+static_assert(sizeof(HostNode<float, 2>) == 20 && sizeof(HostNode<double, 2>) == 40, "reference Node<T,2> layout");
+static_assert(sizeof(HostNode<float, 3>) == 28 && sizeof(HostNode<double, 3>) == 56, "reference Node<T,3> layout");
+
+template <typename T, int kDim> struct HostTree {
+    std::vector<HostNode<T, kDim>> nodes;
+    std::vector<size_t> prim_ids;
+};
 
 template <typename T> struct Handle {
     using U = typename Real<T>::UInt;
@@ -143,8 +152,7 @@ template <typename T> struct Handle {
     DeviceBvh<T> dev;
     bool device_valid = false;
 
-    std::vector<HostNode<T>> nodes;           // reference layout
-    std::vector<size_t> prim_ids;
+    HostTree<T, 3> mirror;
     bool host_valid = false;
     bool maybe_edited = false;                // a mutable node pointer was handed out since the last upload
     uint64_t synced_hash = 0;
@@ -198,12 +206,12 @@ static uint64_t hash_bytes(const void* data, size_t size, uint64_t seed) {
 }
 
 template <typename T> uint64_t ids_hash(const Handle<T>& h) {
-    return hash_bytes(h.prim_ids.data(), h.prim_ids.size() * sizeof(size_t), h.prim_ids.size());
+    return hash_bytes(h.mirror.prim_ids.data(), h.mirror.prim_ids.size() * sizeof(size_t), h.mirror.prim_ids.size());
 }
 
 template <typename T> uint64_t mirror_hash(const Handle<T>& h) {
-    uint64_t a = hash_bytes(h.nodes.data(), h.nodes.size() * sizeof(HostNode<T>), h.nodes.size());
-    return hash_bytes(h.prim_ids.data(), h.prim_ids.size() * sizeof(size_t), a);
+    uint64_t a = hash_bytes(h.mirror.nodes.data(), h.mirror.nodes.size() * sizeof(HostNode<T, 3>), h.mirror.nodes.size());
+    return hash_bytes(h.mirror.prim_ids.data(), h.mirror.prim_ids.size() * sizeof(size_t), a);
 }
 
 // Device -> mirror.  The device array is dense and in the reference's numbering (root at 0, children of a node
@@ -217,16 +225,16 @@ template <typename T> int download_mirror(Handle<T>& h) {
     static_assert(sizeof(size_t) == sizeof(unsigned long long), "prim ids are copied as 64-bit words");
     const size_t node_count = h.dev.node_slots - 1, prim_count = h.dev.prim_count;
     void* d_nodes = nullptr; void* d_ids = nullptr;
-    if (device_alloc(&d_nodes, node_count * sizeof(HostNode<T>), h.stream)) return -1;
+    if (device_alloc(&d_nodes, node_count * sizeof(HostNode<T, 3>), h.stream)) return -1;
     if (device_alloc(&d_ids, prim_count * sizeof(unsigned long long), h.stream)) { device_free(d_nodes, h.stream); return -1; }
     int rc = export_reference_arrays(h.dev, d_nodes, static_cast<unsigned long long*>(d_ids), h.stream);
     if (!rc) {
-        try { h.nodes.resize(node_count); h.prim_ids.resize(prim_count); }
+        try { h.mirror.nodes.resize(node_count); h.mirror.prim_ids.resize(prim_count); }
         catch (const std::exception&) { set_error("download: out of host memory"); rc = -1; }
     }
     cudaError_t err = cudaSuccess;
-    if (!rc) err = cudaMemcpyAsync(h.nodes.data(), d_nodes, node_count * sizeof(HostNode<T>), cudaMemcpyDeviceToHost, h.stream);
-    if (!rc && err == cudaSuccess) err = cudaMemcpyAsync(h.prim_ids.data(), d_ids, prim_count * sizeof(size_t), cudaMemcpyDeviceToHost, h.stream);
+    if (!rc) err = cudaMemcpyAsync(h.mirror.nodes.data(), d_nodes, node_count * sizeof(HostNode<T, 3>), cudaMemcpyDeviceToHost, h.stream);
+    if (!rc && err == cudaSuccess) err = cudaMemcpyAsync(h.mirror.prim_ids.data(), d_ids, prim_count * sizeof(size_t), cudaMemcpyDeviceToHost, h.stream);
     if (!rc && err == cudaSuccess) err = cudaStreamSynchronize(h.stream);
     device_free(d_nodes, h.stream); device_free(d_ids, h.stream);
     if (rc) return -1;
@@ -240,19 +248,20 @@ template <typename T> int download_mirror(Handle<T>& h) {
 // Mirror -> device: reference node i goes to device slot i + 1, padded to 32 / 64 bytes.
 template <typename T> int upload_mirror(Handle<T>& h) {
     BVH_ON_DEVICE(h.device);
-    const size_t node_count = h.nodes.size();
+    const std::vector<HostNode<T, 3>>& nodes = h.mirror.nodes;
+    const size_t node_count = nodes.size();
     if (node_count == 0) { set_error("upload: empty BVH"); return -1; }
     std::vector<DevNode<T>> dev_nodes(node_count + 1);
     std::memset(dev_nodes.data(), 0, sizeof(DevNode<T>));
     for (size_t i = 0; i < node_count; ++i) {
-        std::memcpy(dev_nodes[i + 1].bounds, h.nodes[i].bounds, sizeof(h.nodes[i].bounds));
-        dev_nodes[i + 1].index = h.nodes[i].index;
+        std::memcpy(dev_nodes[i + 1].bounds, nodes[i].bounds, sizeof(nodes[i].bounds));
+        dev_nodes[i + 1].index = nodes[i].index;
         dev_nodes[i + 1].pad = 0;
     }
-    std::vector<uint32_t> ids(h.prim_ids.size());
+    std::vector<uint32_t> ids(h.mirror.prim_ids.size());
     for (size_t i = 0; i < ids.size(); ++i) {
-        if (h.prim_ids[i] >= ids.size()) { set_error("upload: primitive id out of range"); return -1; }
-        ids[i] = (uint32_t)h.prim_ids[i];
+        if (h.mirror.prim_ids[i] >= ids.size()) { set_error("upload: primitive id out of range"); return -1; }
+        ids[i] = (uint32_t)h.mirror.prim_ids[i];
     }
 
     // depth = longest chain of inner nodes (bounds the traversal stack); also validates child indices
@@ -265,12 +274,12 @@ template <typename T> int upload_mirror(Handle<T>& h) {
             auto [i, d] = stack.back();
             stack.pop_back();
             if (++visited > node_count) { set_error("upload: the node graph is not a tree"); return -1; }
-            if (const uint32_t leaf_count = index_count(h.nodes[i].index)) {
+            if (const uint32_t leaf_count = index_count(nodes[i].index)) {
                 // the kernels index tris[first .. first + count) and prim_ids[slot] without further checks
-                if ((size_t)index_first(h.nodes[i].index) + leaf_count > ids.size()) { set_error("upload: leaf range exceeds the primitive count"); return -1; }
+                if ((size_t)index_first(nodes[i].index) + leaf_count > ids.size()) { set_error("upload: leaf range exceeds the primitive count"); return -1; }
                 continue;
             }
-            const size_t first = (size_t)index_first(h.nodes[i].index);
+            const size_t first = (size_t)index_first(nodes[i].index);
             if (first == 0 || first + 1 >= node_count) { set_error("upload: child index out of range"); return -1; }
             depth = std::max(depth, d + 1);
             stack.emplace_back(first, d + 1);
@@ -311,9 +320,31 @@ template <typename T> int ensure_device(Handle<T>& h) {
     return upload_mirror(h);
 }
 
+// A legacy call changed the mirror: the next batched call uploads it.
+template <typename T> void mark_mirror_edited(Handle<T>& h) { h.maybe_edited = true; h.synced_hash = 0; }
+// A batched call changed the device tree: the mirror is stale and is downloaded again when a legacy call needs it.
+template <typename T> void drop_mirror(Handle<T>& h) { h.host_valid = false; h.mirror.nodes.clear(); h.mirror.prim_ids.clear(); }
+
+// The prologue of every entry point that may upload the mirror or enqueue work on the handle's stream: such calls
+// on one handle are serialised (Handle::batch_mutex), run on the handle's device and see a current device tree.
+// `check` returns the error of a call it rejects, before the mirror is uploaded: a rejected call changes nothing.
+// A null handle sets `null_error`, where one is given.
+template <typename T, typename Check, typename Body>
+int on_device_tree(Handle<T>* h, const char* null_error, Check check, Body body) {
+    if (!h) { if (null_error) set_error(null_error); return -1; }
+    std::lock_guard<std::mutex> lock(h->batch_mutex);
+    if (const char* error = check()) { set_error(error); return -1; }
+    BVH_ON_DEVICE(h->device);
+    if (ensure_device(*h)) return -1;
+    return body();
+}
+template <typename T, typename Body> int on_device_tree(Handle<T>* h, const char* null_error, Body body) {
+    return on_device_tree(h, null_error, [] () -> const char* { return nullptr; }, body);
+}
+
 // ---- reference semantics on the mirror ---------------------------------------------------------
 // Bvh::refit with no leaf function (reference bvh.h:184-218; c_api/bvh_impl.h:218-221).
-template <typename T, int kDim, typename NodeVec> void refit_nodes(NodeVec& nodes) {
+template <typename T, int kDim> void refit_nodes(std::vector<HostNode<T, kDim>>& nodes) {
     const size_t n = nodes.size();
     std::vector<size_t> parents(n, 0);
     std::vector<unsigned char> seen(n, 0);
@@ -340,12 +371,11 @@ template <typename T, int kDim, typename NodeVec> void refit_nodes(NodeVec& node
         }
     }
 }
-template <typename T> void refit_mirror(Handle<T>& h) { refit_nodes<T, 3>(h.nodes); }
 
 // Bvh::intersect for one ray with a host callback (reference bvh.h:124-182, c_api/bvh_impl.h:235-250).
-// `nodes` is the mirror in the reference layout (Node<T, kDim>), `ray` = org[kDim] dir[kDim] tmin tmax.
-template <typename T, bool kAny, bool kRobust, int kDim, typename NodeVec, typename Callback>
-void intersect_nodes(const NodeVec& nodes, const T* ray, const Callback* cb) {
+// `ray` = org[kDim] dir[kDim] tmin tmax.
+template <bool kAny, bool kRobust, typename T, int kDim, typename Callback>
+void intersect_nodes(const std::vector<HostNode<T, kDim>>& nodes, const T* ray, const Callback* cb) {
     using U = typename Real<T>::UInt;
     RayCtx<T> r;
     for (int k = 0; k < 3; ++k) { r.org[k] = 0; r.dir[k] = 0; r.inv_dir[k] = 0; r.aux[k] = 0; }
@@ -394,11 +424,6 @@ void intersect_nodes(const NodeVec& nodes, const T* ray, const Callback* cb) {
         if (sp == 0) break;
         top = stack[--sp];
     }
-}
-
-template <typename T, bool kAny, bool kRobust, typename Callback>
-void intersect_mirror(const Handle<T>& h, const T* ray8, const Callback* cb) {
-    intersect_nodes<T, kAny, kRobust, 3>(h.nodes, ray8, cb);
 }
 
 template <typename T> BuildOptions translate_config(const bvh_build_config* config) {
@@ -470,14 +495,9 @@ static unsigned translate_flags(unsigned flags) {
     return tf;
 }
 
+// bvhNN_intersect_rays / _stats after the prologue: the handle's device tree is current.
 template <typename T, typename RayPod, typename HitPod>
-int intersect_batch(Handle<T>* h, const RayPod* rays, size_t n, HitPod* hits, bvh_ray_stats* stats, unsigned flags) {
-    static_assert(sizeof(RayPod) == sizeof(DevRay<T>) && sizeof(HitPod) == sizeof(DevHit<T>), "POD layouts");
-    if (!h) { set_error("null handle"); return -1; }
-    if (n == 0) return 0;
-    std::lock_guard<std::mutex> lock(h->batch_mutex);
-    BVH_ON_DEVICE(h->device);
-    if (ensure_device(*h)) return -1;
+int trace_batch(Handle<T>* h, const RayPod* rays, size_t n, HitPod* hits, bvh_ray_stats* stats, unsigned flags) {
     const unsigned tf = translate_flags(flags);
     if (flags & BVH_DEVICE_POINTERS) {
         return trace_rays<T>(h->dev, reinterpret_cast<const DevRay<T>*>(rays), reinterpret_cast<DevHit<T>*>(hits), n, tf,
@@ -524,22 +544,132 @@ int intersect_batch(Handle<T>* h, const RayPod* rays, size_t n, HitPod* hits, bv
     return check_trace_status(h->dev, h->stream);
 }
 
-// reference bvh.h:220-242 / node.h:90-102: [node_count][prim_count] nodes (6 bounds + index) prim ids
-template <typename T> void save_mirror(Handle<T>& h, FILE* file) {
-    using U = typename Real<T>::UInt;
-    if (download_mirror(h)) return;
-    U v = (U)h.nodes.size(); fwrite(&v, sizeof v, 1, file);
-    v = (U)h.prim_ids.size(); fwrite(&v, sizeof v, 1, file);
-    for (const auto& n : h.nodes) { fwrite(n.bounds, sizeof(T), 6, file); fwrite(&n.index, sizeof(U), 1, file); }
-    for (size_t id : h.prim_ids) { v = (U)id; fwrite(&v, sizeof v, 1, file); }
+template <typename T, typename RayPod, typename HitPod>
+int intersect_batch(Handle<T>* h, const RayPod* rays, size_t n, HitPod* hits, bvh_ray_stats* stats, unsigned flags) {
+    static_assert(sizeof(RayPod) == sizeof(DevRay<T>) && sizeof(HitPod) == sizeof(DevHit<T>), "POD layouts");
+    if (h && n == 0) return 0;
+    return on_device_tree(h, "null handle", [&] { return trace_batch(h, rays, n, hits, stats, flags); });
+}
+template <typename T, typename RayPod, typename HitPod>
+int intersect_batch_stats(Handle<T>* h, const RayPod* rays, size_t n, HitPod* hits, bvh_ray_stats* stats, unsigned flags) {
+    if (!stats) { set_error("stats pointer is null"); return -1; }
+    return intersect_batch(h, rays, n, hits, stats, flags);
+}
+template <typename T>
+int intersect_gather(Handle<T>* h, const DevRay<T>* rays, size_t n, DevHit<T>* hits, void* const* gathered_hits, int world_size,
+                     size_t shard_offset, void* multicast_hits, unsigned flags) {
+    return on_device_tree(h, "null handle", [&] {
+        return !gathered_hits || world_size < 1 || world_size > 8 ? "gather: need 1..8 gathered arrays" : nullptr;
+    }, [&] {
+        GatherTargets g;
+        for (int r = 0; r < 8; ++r) g.peer[r] = r < world_size ? gathered_hits[r] : nullptr;
+        g.count = world_size; g.multicast = multicast_hits; g.offset = shard_offset;
+        return trace_rays<T>(h->dev, rays, hits, n, translate_flags(flags), nullptr, h->stream, &g);
+    });
 }
 
-template <typename T> Handle<T>* load_mirror(FILE* file) {
+// ---- the other 3-D entry points that build or use the device tree ---------------------------------------------
+template <typename T, typename BBox, typename Vec>
+Handle<T>* build_boxes(const BBox* bboxes, const Vec* centers, size_t n, const bvh_build_config* config, unsigned flags) {
+    static_assert(sizeof(BBox) == 6 * sizeof(T) && sizeof(Vec) == 3 * sizeof(T), "box / centre layout");
+    if (!bboxes) { set_error("build_boxes: null boxes"); return nullptr; }
+    if (!centers) { set_error("build_boxes: null centres"); return nullptr; }
+    return build_handle<T>(nullptr, reinterpret_cast<const T*>(bboxes), reinterpret_cast<const T*>(centers), n, config,
+                           (flags & BVH_DEVICE_POINTERS) != 0);
+}
+template <typename T> int set_handle_triangles(Handle<T>* h, const T* vertices, size_t n, unsigned flags) {
+    return on_device_tree(h, "null handle", [&] {
+        if (n != h->dev.prim_count) { set_error("set_triangles: prim_count mismatch"); return -1; }
+        DeviceInput<T> dv(h->stream);
+        if (dv.set(vertices, 9 * n, (flags & BVH_DEVICE_POINTERS) != 0)) return -1;
+        if (attach_triangles<T>(h->dev, dv.ptr, h->stream)) return -1;
+        BVH_CUDA_TRY(cudaStreamSynchronize(h->stream));
+        return 0;
+    });
+}
+template <typename T> int refit_handle_triangles(Handle<T>* h, const T* vertices, size_t n, unsigned flags) {
+    return on_device_tree(h, "null handle", [&] {
+        if (n != h->dev.prim_count) { set_error("refit_triangles: prim_count mismatch"); return -1; }
+        DeviceInput<T> dv(h->stream);
+        if (dv.set(vertices, 9 * n, (flags & BVH_DEVICE_POINTERS) != 0)) return -1;
+        if (refit_triangles<T>(h->dev, dv.ptr, h->stream)) return -1;
+        drop_mirror(*h);
+        BVH_CUDA_TRY(cudaStreamSynchronize(h->stream));
+        return 0;
+    });
+}
+template <typename T, typename BBox> int refit_handle_boxes(Handle<T>* h, const BBox* bboxes, size_t n, unsigned flags) {
+    static_assert(sizeof(BBox) == 6 * sizeof(T), "bbox layout: min3, max3");
+    const bool device_ptrs = (flags & BVH_DEVICE_POINTERS) != 0;
+    return on_device_tree(h, "refit_boxes: null handle", [&] () -> const char* {
+        if (!bboxes) return "refit_boxes: null boxes";
+        if (h->host_valid ? h->mirror.nodes.empty() : !h->device_valid) return "refit_boxes: handle holds no BVH";
+        if (n != (h->host_valid ? h->mirror.prim_ids.size() : (size_t)h->dev.prim_count)) return "refit_boxes: prim_count mismatch";
+        return nullptr;
+    }, [&] {
+        DeviceInput<T> db(h->stream);
+        if (db.set(reinterpret_cast<const T*>(bboxes), 6 * n, device_ptrs)) return -1;
+        if (refit_boxes<T>(h->dev, db.ptr, h->stream)) return -1;
+        drop_mirror(*h);
+        if (!device_ptrs) BVH_CUDA_TRY(cudaStreamSynchronize(h->stream));
+        return 0;
+    });
+}
+template <typename T> int sync_handle(Handle<T>* h) {
+    if (!h) { set_error("null handle"); return -1; }
+    BVH_ON_DEVICE(h->device);
+    return check_trace_status(h->dev, h->stream);
+}
+template <typename T> size_t get_property(Handle<T>* h, int property) {
+    size_t value = (size_t)-1;
+    on_device_tree(h, nullptr, [&] {
+        switch (property) {
+            case BVH_PROP_DEPTH: value = h->dev.depth; break;
+            case BVH_PROP_NODE_SLOTS: value = h->dev.node_slots; break;
+            case BVH_PROP_MORTON_BITS: value = (size_t)h->dev.morton_bits; break;
+            case BVH_PROP_QUALITY: value = (size_t)h->dev.quality; break;
+            case BVH_PROP_TREELETS: value = h->dev.treelets; break;
+            case BVH_PROP_WIDE_NODES: value = h->dev.wide ? h->dev.wide_count : 0; break;
+            case BVH_PROP_LAST_KERNEL: value = (size_t)h->dev.last_kernel; break;
+            case BVH_PROP_STREAM: value = (size_t)reinterpret_cast<uintptr_t>(h->stream); break;
+        }
+        return 0;
+    });
+    return value;
+}
+template <typename T> size_t get_depth(Handle<T>* h) {
+    size_t depth = 0;
+    on_device_tree(h, nullptr, [&] { depth = h->dev.depth; return 0; });
+    return depth;
+}
+template <typename T, typename View> int get_device_view(Handle<T>* h, View* view) {
+    return on_device_tree(h, "get_device_view: null handle", [&] { return view ? nullptr : "get_device_view: null view"; }, [&] {
+        if (!h->dev.nodes || h->dev.node_slots < 2) { set_error("get_device_view: handle holds no BVH"); return -1; }
+        view->device = h->device;
+        view->stream = h->stream;
+        view->nodes = h->dev.nodes;
+        view->prim_ids = h->dev.prim_ids;
+        view->tris = h->dev.tris;
+        view->node_count = h->dev.node_slots - 1;
+        view->prim_count = h->dev.prim_count;
+        view->depth = h->dev.depth;
+        return 0;
+    });
+}
+
+// ---- save / load (reference bvh.h:220-242, node.h:90-102, stream.h) ---------------------------------------------
+// [node_count][prim_count] then per node its 2 * kDim bounds and index, then the primitive ids, all as T / UInt.
+template <typename T, int kDim> void write_tree(const HostTree<T, kDim>& t, FILE* file) {
     using U = typename Real<T>::UInt;
-    DeviceGuard guard(g_device);
-    if (!guard.ok) return nullptr;
-    auto h = new Handle<T>();
-    if (init_handle(*h)) { delete h; return nullptr; }
+    U v = (U)t.nodes.size(); fwrite(&v, sizeof v, 1, file);
+    v = (U)t.prim_ids.size(); fwrite(&v, sizeof v, 1, file);
+    for (const auto& n : t.nodes) { fwrite(n.bounds, sizeof(T), 2 * kDim, file); fwrite(&n.index, sizeof(U), 1, file); }
+    for (size_t id : t.prim_ids) { v = (U)id; fwrite(&v, sizeof v, 1, file); }
+}
+
+template <typename T, int kDim> int read_tree(HostTree<T, kDim>& t, FILE* file) {
+    using U = typename Real<T>::UInt;
+    constexpr size_t kBounds = 2 * kDim;
     U node_count = 0, prim_count = 0;                       // short reads give defaults (stream.h:13-18)
     if (fread(&node_count, sizeof(U), 1, file) != 1) node_count = 0;
     if (fread(&prim_count, sizeof(U), 1, file) != 1) prim_count = 0;
@@ -549,30 +679,51 @@ template <typename T> Handle<T>* load_mirror(FILE* file) {
     if (here >= 0 && fseek(file, 0, SEEK_END) == 0) {
         const long end = ftell(file);
         fseek(file, here, SEEK_SET);
-        const double need = (double)node_count * (6 * sizeof(T) + sizeof(U)) + (double)prim_count * sizeof(U);
-        if (end >= here && need > (double)(end - here)) {
-            set_error("load: the header announces more nodes / primitives than the file holds");
-            destroy_handle(h);
-            return nullptr;
-        }
+        const double need = (double)node_count * (kBounds * sizeof(T) + sizeof(U)) + (double)prim_count * sizeof(U);
+        if (end >= here && need > (double)(end - here)) { set_error("load: the header announces more nodes / primitives than the file holds"); return -1; }
     }
-    try {
-        h->nodes.resize((size_t)node_count);
-        h->prim_ids.resize((size_t)prim_count);
-    } catch (const std::exception&) {
-        set_error("load: out of memory for the announced node / primitive counts");
-        destroy_handle(h);
-        return nullptr;
-    }
-    for (auto& n : h->nodes) {
+    try { t.nodes.resize((size_t)node_count); t.prim_ids.resize((size_t)prim_count); }
+    catch (const std::exception&) { set_error("load: out of memory for the announced node / primitive counts"); return -1; }
+    for (auto& n : t.nodes) {
         std::memset(&n, 0, sizeof n);
-        if (fread(n.bounds, sizeof(T), 6, file) != 6) std::memset(n.bounds, 0, sizeof n.bounds);
+        if (fread(n.bounds, sizeof(T), kBounds, file) != kBounds) std::memset(n.bounds, 0, sizeof n.bounds);
         if (fread(&n.index, sizeof(U), 1, file) != 1) n.index = 0;
     }
-    for (auto& id : h->prim_ids) { U v = 0; if (fread(&v, sizeof(U), 1, file) != 1) v = 0; id = (size_t)v; }
+    for (auto& id : t.prim_ids) { U v = 0; if (fread(&v, sizeof(U), 1, file) != 1) v = 0; id = (size_t)v; }
+    return 0;
+}
+
+template <typename T> void save_handle(Handle<T>& h, FILE* file) { if (!download_mirror(h)) write_tree(h.mirror, file); }
+template <typename T> Handle<T>* load_handle(FILE* file) {
+    DeviceGuard guard(g_device);
+    if (!guard.ok) return nullptr;
+    auto h = new Handle<T>();
+    if (init_handle(*h)) { delete h; return nullptr; }
+    if (read_tree(h->mirror, file)) { destroy_handle(h); return nullptr; }
     h->host_valid = true;
-    h->device_valid = false;
     return h;
+}
+
+// ---- the reference's per-tree calls on the 3-D mirror (downloaded on first use) ---------------------------------
+template <typename T> HostNode<T, 3>* get_node(Handle<T>& h, size_t node_id) {
+    if (download_mirror(h) || node_id >= h.mirror.nodes.size()) return nullptr;
+    if (!h.maybe_edited && h.device_valid) h.synced_hash = mirror_hash(h);
+    h.maybe_edited = true;
+    return &h.mirror.nodes[node_id];
+}
+template <typename T> size_t get_prim_id(Handle<T>& h, size_t i) {
+    return download_mirror(h) || i >= h.mirror.prim_ids.size() ? BVH_INVALID_PRIM_ID : h.mirror.prim_ids[i];
+}
+template <typename T> size_t get_prim_count(const Handle<T>& h) { return h.host_valid ? h.mirror.prim_ids.size() : h.dev.prim_count; }
+template <typename T> size_t get_node_count(Handle<T>& h) { return download_mirror(h) ? 0 : h.mirror.nodes.size(); }
+template <typename T> const size_t* get_prim_ids(Handle<T>* h) { return !h || download_mirror(*h) ? nullptr : h->mirror.prim_ids.data(); }
+template <typename T> void append_node(Handle<T>& h) { if (!download_mirror(h)) { h.mirror.nodes.emplace_back(); mark_mirror_edited(h); } }
+template <typename T> void remove_last_node(Handle<T>& h) {
+    if (!download_mirror(h) && !h.mirror.nodes.empty()) { h.mirror.nodes.pop_back(); mark_mirror_edited(h); }
+}
+template <typename T> void refit(Handle<T>& h) { if (!download_mirror(h)) { refit_nodes(h.mirror.nodes); mark_mirror_edited(h); } }
+template <bool kAny, bool kRobust, typename T, typename Callback> void intersect_ray(Handle<T>& h, const T* ray, const Callback* cb) {
+    if (!download_mirror(h)) intersect_nodes<kAny, kRobust>(h.mirror.nodes, ray, cb);
 }
 
 // ---- 2-D suffixes (reference c_api/bvh.cpp:7-25 instantiates bvh2f / bvh2d next to the 3-D ones) ----------
@@ -581,16 +732,8 @@ template <typename T> Handle<T>* load_mirror(FILE* file) {
 // to z = 0, the LBVH pipeline runs as for 3-D (the z bits of the Morton keys are all zero, so the order is the
 // 2-D Z-curve), and the result comes back as a host tree of the reference's Node<T, 2> (4 bounds + index,
 // 20 / 40 bytes) on which every other entry point works exactly as the reference's does.
-template <typename T> struct HostNode2 { T bounds[4]; typename Real<T>::UInt index; };
-static_assert(sizeof(HostNode2<float>) == 20 && sizeof(HostNode2<double>) == 40, "reference Node<T,2> layout");
-
-template <typename T> struct Handle2 {
-    std::vector<HostNode2<T>> nodes;
-    std::vector<size_t> prim_ids;
-};
-
 template <typename T>
-Handle2<T>* build_handle2(const T* bboxes4, const T* centers2, size_t n, const bvh_build_config* config) {
+HostTree<T, 2>* build_tree2(const T* bboxes4, const T* centers2, size_t n, const bvh_build_config* config) {
     if (n == 0) { set_error("build: prim_count out of range"); return nullptr; }
     std::vector<T> boxes(6 * n), centers(3 * n);
     for (size_t i = 0; i < n; ++i) {                       // bvh_bbox2 = {min.x, min.y, max.x, max.y}
@@ -601,40 +744,50 @@ Handle2<T>* build_handle2(const T* bboxes4, const T* centers2, size_t n, const b
     Handle<T>* lifted = build_handle<T>(nullptr, boxes.data(), centers.data(), n, config, false);
     if (!lifted) return nullptr;
     if (download_mirror(*lifted)) { destroy_handle(lifted); return nullptr; }
-    auto h = new Handle2<T>();
-    h->nodes.resize(lifted->nodes.size());
-    for (size_t i = 0; i < h->nodes.size(); ++i) {
-        std::memcpy(h->nodes[i].bounds, lifted->nodes[i].bounds, 4 * sizeof(T));
-        h->nodes[i].index = lifted->nodes[i].index;
+    auto t = new HostTree<T, 2>();
+    t->nodes.resize(lifted->mirror.nodes.size());
+    for (size_t i = 0; i < t->nodes.size(); ++i) {
+        std::memcpy(t->nodes[i].bounds, lifted->mirror.nodes[i].bounds, 4 * sizeof(T));
+        t->nodes[i].index = lifted->mirror.nodes[i].index;
     }
-    h->prim_ids = lifted->prim_ids;
+    t->prim_ids = lifted->mirror.prim_ids;
     destroy_handle(lifted);
-    return h;
+    return t;
 }
 
-template <typename T> void save_nodes2(const Handle2<T>& h, FILE* file) {
-    using U = typename Real<T>::UInt;
-    U v = (U)h.nodes.size(); fwrite(&v, sizeof v, 1, file);
-    v = (U)h.prim_ids.size(); fwrite(&v, sizeof v, 1, file);
-    for (const auto& n : h.nodes) { fwrite(n.bounds, sizeof(T), 4, file); fwrite(&n.index, sizeof(U), 1, file); }
-    for (size_t id : h.prim_ids) { v = (U)id; fwrite(&v, sizeof v, 1, file); }
+template <typename T> HostTree<T, 2>* load_tree2(FILE* file) {
+    auto t = new HostTree<T, 2>();
+    if (read_tree(*t, file)) { delete t; return nullptr; }
+    return t;
 }
+template <typename T> HostNode<T, 2>* get_node(HostTree<T, 2>& t, size_t node_id) { return node_id < t.nodes.size() ? &t.nodes[node_id] : nullptr; }
+template <typename T> size_t get_prim_id(const HostTree<T, 2>& t, size_t i) { return i < t.prim_ids.size() ? t.prim_ids[i] : BVH_INVALID_PRIM_ID; }
+template <typename T> void remove_last_node(HostTree<T, 2>& t) { if (!t.nodes.empty()) t.nodes.pop_back(); }
 
-template <typename T> Handle2<T>* load_nodes2(FILE* file) {
-    using U = typename Real<T>::UInt;
-    auto h = new Handle2<T>();
-    U node_count = 0, prim_count = 0;
-    if (fread(&node_count, sizeof(U), 1, file) != 1) node_count = 0;
-    if (fread(&prim_count, sizeof(U), 1, file) != 1) prim_count = 0;
-    h->nodes.resize((size_t)node_count);
-    h->prim_ids.resize((size_t)prim_count);
-    for (auto& n : h->nodes) {
-        std::memset(&n, 0, sizeof n);
-        if (fread(n.bounds, sizeof(T), 4, file) != 4) std::memset(n.bounds, 0, sizeof n.bounds);
-        if (fread(&n.index, sizeof(U), 1, file) != 1) n.index = 0;
-    }
-    for (auto& id : h->prim_ids) { U v = 0; if (fread(&v, sizeof(U), 1, file) != 1) v = 0; id = (size_t)v; }
-    return h;
+// ---- the reference's node accessors (c_api/bvh_impl.h) on Node<T, kDim> ------------------------------------------
+template <typename T, int kDim> bool node_is_leaf(const HostNode<T, kDim>* n) { return index_count(n->index) != 0; }
+template <typename T, int kDim> size_t node_prim_count(const HostNode<T, kDim>* n) { return index_count(n->index); }
+template <typename T, int kDim> void set_node_prim_count(HostNode<T, kDim>* n, size_t count) {
+    n->index = make_index(index_first(n->index), (uint32_t)(count & kMaxLeafPrims));
+}
+template <typename T, int kDim> size_t node_first_id(const HostNode<T, kDim>* n) { return (size_t)index_first(n->index); }
+template <typename T, int kDim> void set_node_first_id(HostNode<T, kDim>* n, size_t first_id) {
+    n->index = make_index((typename Real<T>::UInt)first_id, index_count(n->index));
+}
+// bvh_bboxNN is {min[kDim], max[kDim]}; a node interleaves them as min0 max0 min1 max1 ...
+template <typename BBox, typename T, int kDim> BBox node_bbox(const HostNode<T, kDim>* n) {
+    static_assert(sizeof(BBox) == 2 * kDim * sizeof(T), "bbox layout: min[kDim], max[kDim]");
+    T v[2 * kDim];
+    for (int k = 0; k < kDim; ++k) { v[k] = n->bounds[2 * k]; v[kDim + k] = n->bounds[2 * k + 1]; }
+    BBox b;
+    std::memcpy(&b, v, sizeof b);
+    return b;
+}
+template <typename T, int kDim, typename BBox> void set_node_bbox(HostNode<T, kDim>* n, const BBox* bbox) {
+    static_assert(sizeof(BBox) == 2 * kDim * sizeof(T), "bbox layout: min[kDim], max[kDim]");
+    T v[2 * kDim];
+    std::memcpy(v, bbox, sizeof v);
+    for (int k = 0; k < kDim; ++k) { n->bounds[2 * k] = v[k]; n->bounds[2 * k + 1] = v[kDim + k]; }
 }
 
 // bvhNN_optimize (reference c_api/bvh_impl.h:223-233): with a pool the search runs on the pool's thread count
@@ -644,13 +797,29 @@ static size_t optimizer_threads(size_t requested) {
     const unsigned hw = std::thread::hardware_concurrency();
     return hw ? hw : 1;
 }
-template <typename T, int kDim, typename NodeVec>
-bool optimize_nodes(NodeVec& nodes, double ratio, size_t iters, size_t threads) {
-    using NodeT = typename NodeVec::value_type;
+template <typename T, int kDim>
+bool optimize_nodes(std::vector<HostNode<T, kDim>>& nodes, double ratio, size_t iters, size_t threads) {
     try {
-        if (!Reinserter<T, kDim, NodeT>(nodes, threads).run((T)ratio, iters)) { set_error("optimize: the node array is not a well-formed tree"); return false; }
+        if (!Reinserter<T, kDim, HostNode<T, kDim>>(nodes, threads).run((T)ratio, iters)) {
+            set_error("optimize: the node array is not a well-formed tree");
+            return false;
+        }
     } catch (const std::exception& e) { set_error(std::string("optimize: ") + e.what()); return false; }
     return true;
+}
+template <typename T> void optimize(Handle<T>* h, size_t threads) {
+    if (h && !download_mirror(*h) && optimize_nodes(h->mirror.nodes, 0.05, 3, threads)) mark_mirror_edited(*h);
+}
+template <typename T> void optimize(HostTree<T, 2>* t, size_t threads) { if (t) optimize_nodes(t->nodes, 0.05, 3, threads); }
+
+// bvh_optimize_nodes: the Reinserter works on a std::vector; the caller's array is copied in and out (host memory,
+// O(node_count)).
+template <typename T, int kDim> int optimize_array(void* nodes, size_t node_count, double ratio, size_t iters, size_t threads) {
+    HostNode<T, kDim>* first = static_cast<HostNode<T, kDim>*>(nodes);
+    std::vector<HostNode<T, kDim>> v(first, first + node_count);
+    if (!optimize_nodes(v, ratio, iters, optimizer_threads(threads))) return -1;
+    std::copy(v.begin(), v.end(), first);
+    return 0;
 }
 
 } // namespace bvhb200
@@ -708,28 +877,37 @@ static size_t pool_threads(const bvh_thread_pool* pool) { return pool ? optimize
 BVH_EXPORT int bvh_optimize_nodes(void* nodes, size_t node_count, int dim, int is_double, double ratio, size_t iters, size_t threads) {
     if (!nodes && node_count) { set_error("optimize: null node array"); return -1; }
     if (dim != 2 && dim != 3) { set_error("optimize: dim must be 2 or 3"); return -1; }
-    // the Reinserter works on a std::vector; the caller's array is copied in and out (host memory, O(node_count))
-    auto run = [&] (auto tag_node, auto tag_scalar, auto tag_dim) {
-        using NodeT = decltype(tag_node); using T = decltype(tag_scalar); constexpr int D = decltype(tag_dim)::value;
-        std::vector<NodeT> v(static_cast<NodeT*>(nodes), static_cast<NodeT*>(nodes) + node_count);
-        if (!optimize_nodes<T, D>(v, ratio, iters, optimizer_threads(threads))) return -1;
-        std::memcpy(nodes, v.data(), node_count * sizeof(NodeT));
-        return 0;
-    };
     try {
-        if (dim == 3) return is_double ? run(HostNode<double>{}, double{}, std::integral_constant<int, 3>{})
-                                       : run(HostNode<float>{}, float{}, std::integral_constant<int, 3>{});
-        return is_double ? run(HostNode2<double>{}, double{}, std::integral_constant<int, 2>{})
-                         : run(HostNode2<float>{}, float{}, std::integral_constant<int, 2>{});
+        if (dim == 3) return is_double ? optimize_array<double, 3>(nodes, node_count, ratio, iters, threads)
+                                       : optimize_array<float, 3>(nodes, node_count, ratio, iters, threads);
+        return is_double ? optimize_array<double, 2>(nodes, node_count, ratio, iters, threads)
+                         : optimize_array<float, 2>(nodes, node_count, ratio, iters, threads);
     } catch (const std::exception& e) { set_error(std::string("optimize: ") + e.what()); return -1; }
 }
 BVH_EXPORT struct bvh_thread_pool* bvh_thread_pool_create(size_t thread_count) { return new bvh_thread_pool { thread_count }; }
 BVH_EXPORT void bvh_thread_pool_destroy(struct bvh_thread_pool* pool) { delete pool; }
 
+// The exported functions below only convert their arguments and call the templates above.
 #define H(T, bvh) (reinterpret_cast<Handle<T>*>(bvh))
 #define HC(T, bvh) (const_cast<Handle<T>*>(reinterpret_cast<const Handle<T>*>(bvh)))
-#define N(T, node) (reinterpret_cast<HostNode<T>*>(node))
-#define NC(T, node) (reinterpret_cast<const HostNode<T>*>(node))
+#define H2(T, bvh) (reinterpret_cast<HostTree<T, 2>*>(bvh))
+#define HC2(T, bvh) (reinterpret_cast<const HostTree<T, 2>*>(bvh))
+#define N(T, D, node) (reinterpret_cast<HostNode<T, D>*>(node))
+#define NC(T, D, node) (reinterpret_cast<const HostNode<T, D>*>(node))
+
+#define BVH_IMPL_NODE(T, D, S)                                                                                     \
+    BVH_EXPORT bool bvh_node##S##_is_leaf(const struct bvh_node##S* node) { return node_is_leaf(NC(T, D, node)); } \
+    BVH_EXPORT size_t bvh_node##S##_get_prim_count(const struct bvh_node##S* node) { return node_prim_count(NC(T, D, node)); } \
+    BVH_EXPORT void bvh_node##S##_set_prim_count(struct bvh_node##S* node, size_t count) { set_node_prim_count(N(T, D, node), count); } \
+    BVH_EXPORT size_t bvh_node##S##_get_first_id(const struct bvh_node##S* node) { return node_first_id(NC(T, D, node)); } \
+    BVH_EXPORT void bvh_node##S##_set_first_id(struct bvh_node##S* node, size_t first_id) { set_node_first_id(N(T, D, node), first_id); } \
+    BVH_EXPORT struct bvh_bbox##S bvh_node##S##_get_bbox(const struct bvh_node##S* node) { return node_bbox<bvh_bbox##S>(NC(T, D, node)); } \
+    BVH_EXPORT void bvh_node##S##_set_bbox(struct bvh_node##S* node, const struct bvh_bbox##S* bbox) { set_node_bbox(N(T, D, node), bbox); }
+
+BVH_IMPL_NODE(float, 2, 2f)
+BVH_IMPL_NODE(float, 3, 3f)
+BVH_IMPL_NODE(double, 2, 2d)
+BVH_IMPL_NODE(double, 3, 3d)
 
 #define BVH_IMPL_3D(T, S, CALLBACK)                                                                               \
     BVH_EXPORT struct bvh##S* bvh##S##_build(struct bvh_thread_pool*, const struct bvh_bbox##S* bboxes,            \
@@ -744,265 +922,79 @@ BVH_EXPORT void bvh_thread_pool_destroy(struct bvh_thread_pool* pool) { delete p
     }                                                                                                              \
     BVH_EXPORT struct bvh##S* bvh##S##_build_boxes(const struct bvh_bbox##S* bboxes, const struct bvh_vec##S* centers, \
             size_t prim_count, const struct bvh_build_config* config, unsigned flags) {                            \
-        static_assert(sizeof(bvh_bbox##S) == 6 * sizeof(T) && sizeof(bvh_vec##S) == 3 * sizeof(T), "box / centre layout"); \
-        if (!bboxes) { set_error("build_boxes: null boxes"); return nullptr; }                                     \
-        if (!centers) { set_error("build_boxes: null centres"); return nullptr; }                                  \
-        return reinterpret_cast<bvh##S*>(build_handle<T>(nullptr, reinterpret_cast<const T*>(bboxes),              \
-            reinterpret_cast<const T*>(centers), prim_count, config, (flags & BVH_DEVICE_POINTERS) != 0));         \
-    }                                                                                                              \
+        return reinterpret_cast<bvh##S*>(build_boxes<T>(bboxes, centers, prim_count, config, flags)); }            \
     BVH_EXPORT void bvh##S##_destroy(struct bvh##S* bvh) { destroy_handle(H(T, bvh)); }                            \
-    BVH_EXPORT void bvh##S##_save(const struct bvh##S* bvh, FILE* file) { save_mirror(*HC(T, bvh), file); }        \
-    BVH_EXPORT struct bvh##S* bvh##S##_load(FILE* file) { return reinterpret_cast<bvh##S*>(load_mirror<T>(file)); } \
+    BVH_EXPORT void bvh##S##_save(const struct bvh##S* bvh, FILE* file) { save_handle(*HC(T, bvh), file); }        \
+    BVH_EXPORT struct bvh##S* bvh##S##_load(FILE* file) { return reinterpret_cast<bvh##S*>(load_handle<T>(file)); } \
     BVH_EXPORT struct bvh_node##S* bvh##S##_get_node(struct bvh##S* bvh, size_t node_id) {                         \
-        auto h = H(T, bvh);                                                                                        \
-        if (download_mirror(*h) || node_id >= h->nodes.size()) return nullptr;                                     \
-        if (!h->maybe_edited && h->device_valid) h->synced_hash = mirror_hash(*h);                                 \
-        h->maybe_edited = true;                                                                                    \
-        return reinterpret_cast<bvh_node##S*>(&h->nodes[node_id]);                                                 \
-    }                                                                                                              \
-    BVH_EXPORT size_t bvh##S##_get_prim_id(const struct bvh##S* bvh, size_t i) {                                   \
-        auto h = HC(T, bvh);                                                                                       \
-        if (download_mirror(*h) || i >= h->prim_ids.size()) return BVH_INVALID_PRIM_ID;                            \
-        return h->prim_ids[i];                                                                                     \
-    }                                                                                                              \
-    BVH_EXPORT size_t bvh##S##_get_prim_count(const struct bvh##S* bvh) {                                          \
-        auto h = HC(T, bvh);                                                                                       \
-        return h->host_valid ? h->prim_ids.size() : h->dev.prim_count;                                             \
-    }                                                                                                              \
-    BVH_EXPORT size_t bvh##S##_get_node_count(const struct bvh##S* bvh) {                                          \
-        auto h = HC(T, bvh);                                                                                       \
-        return download_mirror(*h) ? 0 : h->nodes.size();                                                          \
-    }                                                                                                              \
-    BVH_EXPORT bool bvh_node##S##_is_leaf(const struct bvh_node##S* node) { return index_count(NC(T, node)->index) != 0; } \
-    BVH_EXPORT size_t bvh_node##S##_get_prim_count(const struct bvh_node##S* node) { return index_count(NC(T, node)->index); } \
-    BVH_EXPORT void bvh_node##S##_set_prim_count(struct bvh_node##S* node, size_t count) {                         \
-        using U = Real<T>::UInt;                                                                                   \
-        N(T, node)->index = make_index<U>(index_first(N(T, node)->index), (uint32_t)(count & kMaxLeafPrims));      \
-    }                                                                                                              \
-    BVH_EXPORT size_t bvh_node##S##_get_first_id(const struct bvh_node##S* node) { return (size_t)index_first(NC(T, node)->index); } \
-    BVH_EXPORT void bvh_node##S##_set_first_id(struct bvh_node##S* node, size_t first_id) {                        \
-        using U = Real<T>::UInt;                                                                                   \
-        N(T, node)->index = make_index<U>((U)first_id, index_count(N(T, node)->index));                            \
-    }                                                                                                              \
-    BVH_EXPORT struct bvh_bbox##S bvh_node##S##_get_bbox(const struct bvh_node##S* node) {                         \
-        const T* b = NC(T, node)->bounds;                                                                          \
-        return bvh_bbox##S { { b[0], b[2], b[4] }, { b[1], b[3], b[5] } };                                         \
-    }                                                                                                              \
-    BVH_EXPORT void bvh_node##S##_set_bbox(struct bvh_node##S* node, const struct bvh_bbox##S* bbox) {             \
-        T* b = N(T, node)->bounds;                                                                                 \
-        b[0] = bbox->min.x; b[1] = bbox->max.x; b[2] = bbox->min.y; b[3] = bbox->max.y; b[4] = bbox->min.z; b[5] = bbox->max.z; \
-    }                                                                                                              \
-    BVH_EXPORT void bvh##S##_append_node(struct bvh##S* bvh) {                                                     \
-        auto h = H(T, bvh);                                                                                        \
-        if (download_mirror(*h)) return;                                                                           \
-        h->nodes.emplace_back(); h->maybe_edited = true; h->synced_hash = 0;                                       \
-    }                                                                                                              \
-    BVH_EXPORT void bvh##S##_remove_last_node(struct bvh##S* bvh) {                                                \
-        auto h = H(T, bvh);                                                                                        \
-        if (download_mirror(*h) || h->nodes.empty()) return;                                                       \
-        h->nodes.pop_back(); h->maybe_edited = true; h->synced_hash = 0;                                           \
-    }                                                                                                              \
-    BVH_EXPORT void bvh##S##_refit(struct bvh##S* bvh) {                                                           \
-        auto h = H(T, bvh);                                                                                        \
-        if (download_mirror(*h)) return;                                                                           \
-        refit_mirror(*h); h->maybe_edited = true; h->synced_hash = 0;                                              \
-    }                                                                                                              \
-    BVH_EXPORT void bvh##S##_optimize(struct bvh_thread_pool* pool, struct bvh##S* bvh) {                          \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h || download_mirror(*h)) return;                                                                     \
-        if (optimize_nodes<T, 3>(h->nodes, 0.05, 3, pool_threads(pool))) { h->maybe_edited = true; h->synced_hash = 0; } \
-    }                                                                                                              \
+        return reinterpret_cast<bvh_node##S*>(get_node(*H(T, bvh), node_id)); }                                    \
+    BVH_EXPORT size_t bvh##S##_get_prim_id(const struct bvh##S* bvh, size_t i) { return get_prim_id(*HC(T, bvh), i); } \
+    BVH_EXPORT size_t bvh##S##_get_prim_count(const struct bvh##S* bvh) { return get_prim_count(*HC(T, bvh)); }    \
+    BVH_EXPORT size_t bvh##S##_get_node_count(const struct bvh##S* bvh) { return get_node_count(*HC(T, bvh)); }    \
+    BVH_EXPORT void bvh##S##_append_node(struct bvh##S* bvh) { append_node(*H(T, bvh)); }                          \
+    BVH_EXPORT void bvh##S##_remove_last_node(struct bvh##S* bvh) { remove_last_node(*H(T, bvh)); }                \
+    BVH_EXPORT void bvh##S##_refit(struct bvh##S* bvh) { refit(*H(T, bvh)); }                                      \
+    BVH_EXPORT void bvh##S##_optimize(struct bvh_thread_pool* pool, struct bvh##S* bvh) { optimize(H(T, bvh), pool_threads(pool)); } \
     BVH_EXPORT void bvh##S##_intersect_ray_any(const struct bvh##S* bvh, const struct bvh_ray##S* ray, const struct CALLBACK* cb) { \
-        auto h = HC(T, bvh); if (!download_mirror(*h)) intersect_mirror<T, true, false>(*h, reinterpret_cast<const T*>(ray), cb); } \
+        intersect_ray<true, false>(*HC(T, bvh), reinterpret_cast<const T*>(ray), cb); }                           \
     BVH_EXPORT void bvh##S##_intersect_ray_any_robust(const struct bvh##S* bvh, const struct bvh_ray##S* ray, const struct CALLBACK* cb) { \
-        auto h = HC(T, bvh); if (!download_mirror(*h)) intersect_mirror<T, true, true>(*h, reinterpret_cast<const T*>(ray), cb); } \
+        intersect_ray<true, true>(*HC(T, bvh), reinterpret_cast<const T*>(ray), cb); }                            \
     BVH_EXPORT void bvh##S##_intersect_ray(const struct bvh##S* bvh, const struct bvh_ray##S* ray, const struct CALLBACK* cb) { \
-        auto h = HC(T, bvh); if (!download_mirror(*h)) intersect_mirror<T, false, false>(*h, reinterpret_cast<const T*>(ray), cb); } \
+        intersect_ray<false, false>(*HC(T, bvh), reinterpret_cast<const T*>(ray), cb); }                          \
     BVH_EXPORT void bvh##S##_intersect_ray_robust(const struct bvh##S* bvh, const struct bvh_ray##S* ray, const struct CALLBACK* cb) { \
-        auto h = HC(T, bvh); if (!download_mirror(*h)) intersect_mirror<T, false, true>(*h, reinterpret_cast<const T*>(ray), cb); } \
+        intersect_ray<false, true>(*HC(T, bvh), reinterpret_cast<const T*>(ray), cb); }                           \
     BVH_EXPORT int bvh##S##_set_triangles(struct bvh##S* bvh, const T* vertices, size_t prim_count, unsigned flags) { \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h) { set_error("null handle"); return -1; }                                                           \
-        BVH_ON_DEVICE(h->device);                                                                    \
-        if (ensure_device(*h)) return -1;                                                                          \
-        if (prim_count != h->dev.prim_count) { set_error("set_triangles: prim_count mismatch"); return -1; }       \
-        DeviceInput<T> dv(h->stream);                                                                              \
-        if (dv.set(vertices, 9 * prim_count, (flags & BVH_DEVICE_POINTERS) != 0)) return -1;                       \
-        if (attach_triangles<T>(h->dev, dv.ptr, h->stream)) return -1;                                             \
-        BVH_CUDA_TRY(cudaStreamSynchronize(h->stream));                                                            \
-        return 0;                                                                                                  \
-    }                                                                                                              \
+        return set_handle_triangles(H(T, bvh), vertices, prim_count, flags); }                                     \
     BVH_EXPORT int bvh##S##_refit_triangles(struct bvh##S* bvh, const T* vertices, size_t prim_count, unsigned flags) { \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h) { set_error("null handle"); return -1; }                                                           \
-        BVH_ON_DEVICE(h->device);                                                                    \
-        if (ensure_device(*h)) return -1;                                                                          \
-        if (prim_count != h->dev.prim_count) { set_error("refit_triangles: prim_count mismatch"); return -1; }     \
-        DeviceInput<T> dv(h->stream);                                                                              \
-        if (dv.set(vertices, 9 * prim_count, (flags & BVH_DEVICE_POINTERS) != 0)) return -1;                       \
-        if (refit_triangles<T>(h->dev, dv.ptr, h->stream)) return -1;                                              \
-        h->host_valid = false;                   /* the mirror (if any) is stale: re-download on demand */        \
-        h->nodes.clear(); h->prim_ids.clear();                                                                     \
-        BVH_CUDA_TRY(cudaStreamSynchronize(h->stream));                                                            \
-        return 0;                                                                                                  \
-    }                                                                                                              \
-    BVH_EXPORT int bvh##S##_refit_boxes(struct bvh##S* bvh, const struct bvh_bbox##S* bboxes, size_t prim_count,   \
-            unsigned flags) {                                                                                      \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h) { set_error("refit_boxes: null handle"); return -1; }                                              \
-        if (!bboxes) { set_error("refit_boxes: null boxes"); return -1; }                                         \
-        static_assert(sizeof(bvh_bbox##S) == 6 * sizeof(T), "bbox layout: min3, max3");                            \
-        std::lock_guard<std::mutex> lock(h->batch_mutex);                                                          \
-        /* checked before ensure_device, so that a failed call changes nothing on the device */                   \
-        if (h->host_valid ? h->nodes.empty() : !h->device_valid) { set_error("refit_boxes: handle holds no BVH"); return -1; } \
-        if (prim_count != (h->host_valid ? h->prim_ids.size() : (size_t)h->dev.prim_count)) {                     \
-            set_error("refit_boxes: prim_count mismatch"); return -1;                                              \
-        }                                                                                                          \
-        BVH_ON_DEVICE(h->device);                                                                                  \
-        if (ensure_device(*h)) return -1;                                                                          \
-        const bool device_ptrs = (flags & BVH_DEVICE_POINTERS) != 0;                                               \
-        DeviceInput<T> db(h->stream);                                                                              \
-        if (db.set(reinterpret_cast<const T*>(bboxes), 6 * prim_count, device_ptrs)) return -1;                   \
-        if (refit_boxes<T>(h->dev, db.ptr, h->stream)) return -1;                                                  \
-        h->host_valid = false;                   /* the mirror (if any) is stale: re-download on demand */        \
-        h->nodes.clear(); h->prim_ids.clear();                                                                     \
-        if (!device_ptrs) BVH_CUDA_TRY(cudaStreamSynchronize(h->stream));                                          \
-        return 0;                                                                                                  \
-    }                                                                                                              \
+        return refit_handle_triangles(H(T, bvh), vertices, prim_count, flags); }                                   \
+    BVH_EXPORT int bvh##S##_refit_boxes(struct bvh##S* bvh, const struct bvh_bbox##S* bboxes, size_t prim_count, unsigned flags) { \
+        return refit_handle_boxes(H(T, bvh), bboxes, prim_count, flags); }                                         \
     BVH_EXPORT int bvh##S##_intersect_rays(struct bvh##S* bvh, const struct bvh_ray##S* rays, size_t ray_count,    \
             struct bvh_hit##S* hits, unsigned flags) {                                                             \
-        return intersect_batch<T>(H(T, bvh), rays, ray_count, hits, nullptr, flags);                               \
-    }                                                                                                              \
+        return intersect_batch<T>(H(T, bvh), rays, ray_count, hits, nullptr, flags); }                             \
     BVH_EXPORT int bvh##S##_intersect_rays_gather(struct bvh##S* bvh, const struct bvh_ray##S* rays, size_t ray_count, \
             struct bvh_hit##S* hits, void* const* gathered_hits, int world_size, size_t shard_offset,              \
             void* multicast_hits, unsigned flags) {                                                                \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h) { set_error("null handle"); return -1; }                                                           \
-        if (!gathered_hits || world_size < 1 || world_size > 8) { set_error("gather: need 1..8 gathered arrays"); return -1; } \
-        std::lock_guard<std::mutex> lock(h->batch_mutex);                                                          \
-        BVH_ON_DEVICE(h->device);                                                                    \
-        if (ensure_device(*h)) return -1;                                                                          \
-        GatherTargets g;                                                                                           \
-        for (int r = 0; r < 8; ++r) g.peer[r] = r < world_size ? gathered_hits[r] : nullptr;                      \
-        g.count = world_size; g.multicast = multicast_hits; g.offset = shard_offset;                               \
-        return trace_rays<T>(h->dev, reinterpret_cast<const DevRay<T>*>(rays), reinterpret_cast<DevHit<T>*>(hits), \
-                             ray_count, translate_flags(flags), nullptr, h->stream, &g);                           \
-    }                                                                                                              \
+        return intersect_gather(H(T, bvh), reinterpret_cast<const DevRay<T>*>(rays), ray_count,                    \
+            reinterpret_cast<DevHit<T>*>(hits), gathered_hits, world_size, shard_offset, multicast_hits, flags); } \
     BVH_EXPORT int bvh##S##_intersect_rays_stats(struct bvh##S* bvh, const struct bvh_ray##S* rays, size_t ray_count, \
             struct bvh_hit##S* hits, struct bvh_ray_stats* stats, unsigned flags) {                                \
-        if (!stats) { set_error("stats pointer is null"); return -1; }                                             \
-        return intersect_batch<T>(H(T, bvh), rays, ray_count, hits, stats, flags);                                 \
-    }                                                                                                              \
-    BVH_EXPORT int bvh##S##_sync(struct bvh##S* bvh) {                                                             \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h) { set_error("null handle"); return -1; }                                                           \
-        BVH_ON_DEVICE(h->device);                                                                    \
-        return check_trace_status(h->dev, h->stream);                                                              \
-    }                                                                                                              \
-    BVH_EXPORT size_t bvh##S##_get_depth(struct bvh##S* bvh) {                                                     \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h || ensure_device(*h)) return 0;                                                                     \
-        return h->dev.depth;                                                                                       \
-    }                                                                                                              \
-    BVH_EXPORT const size_t* bvh##S##_get_prim_ids(struct bvh##S* bvh) {                                           \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h || download_mirror(*h)) return nullptr;                                                             \
-        return h->prim_ids.data();                                                                                 \
-    }                                                                                                              \
-    BVH_EXPORT size_t bvh##S##_get_property(struct bvh##S* bvh, int property) {                                    \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h || ensure_device(*h)) return (size_t)-1;                                                            \
-        switch (property) {                                                                                        \
-            case BVH_PROP_DEPTH: return h->dev.depth;                                                              \
-            case BVH_PROP_NODE_SLOTS: return h->dev.node_slots;                                                    \
-            case BVH_PROP_MORTON_BITS: return (size_t)h->dev.morton_bits;                                          \
-            case BVH_PROP_QUALITY: return (size_t)h->dev.quality;                                                  \
-            case BVH_PROP_TREELETS: return h->dev.treelets;                                                        \
-            case BVH_PROP_WIDE_NODES: return h->dev.wide ? h->dev.wide_count : 0;                                  \
-            case BVH_PROP_LAST_KERNEL: return (size_t)h->dev.last_kernel;                                          \
-            case BVH_PROP_STREAM: return (size_t)reinterpret_cast<uintptr_t>(h->stream);                           \
-            default: return (size_t)-1;                                                                            \
-        }                                                                                                          \
-    }                                                                                                              \
-    BVH_EXPORT int bvh##S##_get_device_view(struct bvh##S* bvh, struct bvh_device_view##S* view) {                 \
-        auto h = H(T, bvh);                                                                                        \
-        if (!h) { set_error("get_device_view: null handle"); return -1; }                                          \
-        if (!view) { set_error("get_device_view: null view"); return -1; }                                         \
-        std::lock_guard<std::mutex> lock(h->batch_mutex);                                                          \
-        BVH_ON_DEVICE(h->device);                                                                                  \
-        if (ensure_device(*h)) return -1;                                                                          \
-        if (!h->dev.nodes || h->dev.node_slots < 2) { set_error("get_device_view: handle holds no BVH"); return -1; } \
-        view->device = h->device;                                                                                  \
-        view->stream = h->stream;                                                                                  \
-        view->nodes = h->dev.nodes;                                                                                \
-        view->prim_ids = h->dev.prim_ids;                                                                          \
-        view->tris = h->dev.tris;                                                                                  \
-        view->node_count = h->dev.node_slots - 1;                                                                  \
-        view->prim_count = h->dev.prim_count;                                                                      \
-        view->depth = h->dev.depth;                                                                                \
-        return 0;                                                                                                  \
-    }
+        return intersect_batch_stats<T>(H(T, bvh), rays, ray_count, hits, stats, flags); }                         \
+    BVH_EXPORT int bvh##S##_sync(struct bvh##S* bvh) { return sync_handle(H(T, bvh)); }                            \
+    BVH_EXPORT size_t bvh##S##_get_depth(struct bvh##S* bvh) { return get_depth(H(T, bvh)); }                      \
+    BVH_EXPORT const size_t* bvh##S##_get_prim_ids(struct bvh##S* bvh) { return get_prim_ids(H(T, bvh)); }         \
+    BVH_EXPORT size_t bvh##S##_get_property(struct bvh##S* bvh, int property) { return get_property(H(T, bvh), property); } \
+    BVH_EXPORT int bvh##S##_get_device_view(struct bvh##S* bvh, struct bvh_device_view##S* view) { return get_device_view(H(T, bvh), view); }
 
 BVH_IMPL_3D(float, 3f, bvh_intersect_callbackf)
 BVH_IMPL_3D(double, 3d, bvh_intersect_callbackd)
 
-#define H2(T, bvh) (reinterpret_cast<Handle2<T>*>(bvh))
-#define HC2(T, bvh) (reinterpret_cast<const Handle2<T>*>(bvh))
-#define N2(T, node) (reinterpret_cast<HostNode2<T>*>(node))
-#define NC2(T, node) (reinterpret_cast<const HostNode2<T>*>(node))
-
 #define BVH_IMPL_2D(T, S, CALLBACK)                                                                                \
     BVH_EXPORT struct bvh##S* bvh##S##_build(struct bvh_thread_pool*, const struct bvh_bbox##S* bboxes,            \
             const struct bvh_vec##S* centers, size_t prim_count, const struct bvh_build_config* config) {          \
-        return reinterpret_cast<bvh##S*>(build_handle2<T>(reinterpret_cast<const T*>(bboxes),                      \
+        return reinterpret_cast<bvh##S*>(build_tree2<T>(reinterpret_cast<const T*>(bboxes),                        \
             reinterpret_cast<const T*>(centers), prim_count, config));                                             \
     }                                                                                                              \
     BVH_EXPORT void bvh##S##_destroy(struct bvh##S* bvh) { delete H2(T, bvh); }                                    \
-    BVH_EXPORT void bvh##S##_save(const struct bvh##S* bvh, FILE* file) { save_nodes2(*HC2(T, bvh), file); }       \
-    BVH_EXPORT struct bvh##S* bvh##S##_load(FILE* file) { return reinterpret_cast<bvh##S*>(load_nodes2<T>(file)); } \
+    BVH_EXPORT void bvh##S##_save(const struct bvh##S* bvh, FILE* file) { write_tree(*HC2(T, bvh), file); }        \
+    BVH_EXPORT struct bvh##S* bvh##S##_load(FILE* file) { return reinterpret_cast<bvh##S*>(load_tree2<T>(file)); } \
     BVH_EXPORT struct bvh_node##S* bvh##S##_get_node(struct bvh##S* bvh, size_t node_id) {                         \
-        auto h = H2(T, bvh);                                                                                       \
-        return node_id < h->nodes.size() ? reinterpret_cast<bvh_node##S*>(&h->nodes[node_id]) : nullptr;           \
-    }                                                                                                              \
-    BVH_EXPORT size_t bvh##S##_get_prim_id(const struct bvh##S* bvh, size_t i) {                                   \
-        auto h = HC2(T, bvh);                                                                                      \
-        return i < h->prim_ids.size() ? h->prim_ids[i] : BVH_INVALID_PRIM_ID;                                      \
-    }                                                                                                              \
+        return reinterpret_cast<bvh_node##S*>(get_node(*H2(T, bvh), node_id)); }                                   \
+    BVH_EXPORT size_t bvh##S##_get_prim_id(const struct bvh##S* bvh, size_t i) { return get_prim_id(*HC2(T, bvh), i); } \
     BVH_EXPORT size_t bvh##S##_get_prim_count(const struct bvh##S* bvh) { return HC2(T, bvh)->prim_ids.size(); }   \
     BVH_EXPORT size_t bvh##S##_get_node_count(const struct bvh##S* bvh) { return HC2(T, bvh)->nodes.size(); }      \
-    BVH_EXPORT bool bvh_node##S##_is_leaf(const struct bvh_node##S* node) { return index_count(NC2(T, node)->index) != 0; } \
-    BVH_EXPORT size_t bvh_node##S##_get_prim_count(const struct bvh_node##S* node) { return index_count(NC2(T, node)->index); } \
-    BVH_EXPORT void bvh_node##S##_set_prim_count(struct bvh_node##S* node, size_t count) {                         \
-        using U = Real<T>::UInt;                                                                                   \
-        N2(T, node)->index = make_index<U>(index_first(N2(T, node)->index), (uint32_t)(count & kMaxLeafPrims));    \
-    }                                                                                                              \
-    BVH_EXPORT size_t bvh_node##S##_get_first_id(const struct bvh_node##S* node) { return (size_t)index_first(NC2(T, node)->index); } \
-    BVH_EXPORT void bvh_node##S##_set_first_id(struct bvh_node##S* node, size_t first_id) {                        \
-        using U = Real<T>::UInt;                                                                                   \
-        N2(T, node)->index = make_index<U>((U)first_id, index_count(N2(T, node)->index));                          \
-    }                                                                                                              \
-    BVH_EXPORT struct bvh_bbox##S bvh_node##S##_get_bbox(const struct bvh_node##S* node) {                         \
-        const T* b = NC2(T, node)->bounds;                                                                         \
-        return bvh_bbox##S { { b[0], b[2] }, { b[1], b[3] } };                                                     \
-    }                                                                                                              \
-    BVH_EXPORT void bvh_node##S##_set_bbox(struct bvh_node##S* node, const struct bvh_bbox##S* bbox) {             \
-        T* b = N2(T, node)->bounds;                                                                                \
-        b[0] = bbox->min.x; b[1] = bbox->max.x; b[2] = bbox->min.y; b[3] = bbox->max.y;                            \
-    }                                                                                                              \
     BVH_EXPORT void bvh##S##_append_node(struct bvh##S* bvh) { H2(T, bvh)->nodes.emplace_back(); }                 \
-    BVH_EXPORT void bvh##S##_remove_last_node(struct bvh##S* bvh) { if (!H2(T, bvh)->nodes.empty()) H2(T, bvh)->nodes.pop_back(); } \
-    BVH_EXPORT void bvh##S##_refit(struct bvh##S* bvh) { refit_nodes<T, 2>(H2(T, bvh)->nodes); }                   \
-    BVH_EXPORT void bvh##S##_optimize(struct bvh_thread_pool* pool, struct bvh##S* bvh) {                          \
-        if (bvh) optimize_nodes<T, 2>(H2(T, bvh)->nodes, 0.05, 3, pool_threads(pool));                             \
-    }                                                                                                              \
+    BVH_EXPORT void bvh##S##_remove_last_node(struct bvh##S* bvh) { remove_last_node(*H2(T, bvh)); }               \
+    BVH_EXPORT void bvh##S##_refit(struct bvh##S* bvh) { refit_nodes(H2(T, bvh)->nodes); }                         \
+    BVH_EXPORT void bvh##S##_optimize(struct bvh_thread_pool* pool, struct bvh##S* bvh) { optimize(H2(T, bvh), pool_threads(pool)); } \
     BVH_EXPORT void bvh##S##_intersect_ray_any(const struct bvh##S* bvh, const struct bvh_ray##S* ray, const struct CALLBACK* cb) { \
-        intersect_nodes<T, true, false, 2>(HC2(T, bvh)->nodes, reinterpret_cast<const T*>(ray), cb); }            \
+        intersect_nodes<true, false>(HC2(T, bvh)->nodes, reinterpret_cast<const T*>(ray), cb); }                  \
     BVH_EXPORT void bvh##S##_intersect_ray_any_robust(const struct bvh##S* bvh, const struct bvh_ray##S* ray, const struct CALLBACK* cb) { \
-        intersect_nodes<T, true, true, 2>(HC2(T, bvh)->nodes, reinterpret_cast<const T*>(ray), cb); }             \
+        intersect_nodes<true, true>(HC2(T, bvh)->nodes, reinterpret_cast<const T*>(ray), cb); }                   \
     BVH_EXPORT void bvh##S##_intersect_ray(const struct bvh##S* bvh, const struct bvh_ray##S* ray, const struct CALLBACK* cb) { \
-        intersect_nodes<T, false, false, 2>(HC2(T, bvh)->nodes, reinterpret_cast<const T*>(ray), cb); }           \
+        intersect_nodes<false, false>(HC2(T, bvh)->nodes, reinterpret_cast<const T*>(ray), cb); }                 \
     BVH_EXPORT void bvh##S##_intersect_ray_robust(const struct bvh##S* bvh, const struct bvh_ray##S* ray, const struct CALLBACK* cb) { \
-        intersect_nodes<T, false, true, 2>(HC2(T, bvh)->nodes, reinterpret_cast<const T*>(ray), cb); }
+        intersect_nodes<false, true>(HC2(T, bvh)->nodes, reinterpret_cast<const T*>(ray), cb); }
 
 BVH_IMPL_2D(float, 2f, bvh_intersect_callbackf)
 BVH_IMPL_2D(double, 2d, bvh_intersect_callbackd)
