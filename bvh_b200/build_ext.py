@@ -70,6 +70,8 @@ BOTTOM_UP_KERNELS_SRC = os.path.join(ROOT, "tests", "device_bottom_up_kernels.cu
 BOTTOM_UP_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_bottom_up_kernels.so")
 TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_trace_kernels.cu")
 TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_trace_kernels.so")
+QUERY_BATCH_KERNELS_SRC = os.path.join(ROOT, "tests", "device_query_batch_kernels.cu")
+QUERY_BATCH_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_query_batch_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -118,6 +120,12 @@ def build_device_trace_tests(force: bool = False, verbose: bool = False) -> str:
     """tests/device_trace_kernels.cu: the test tracers of DeviceView::trace (triangles, spheres, leaf-call recorders)
     and the same tracers one thread per ray."""
     return _build_test_kernels(TRACE_KERNELS_SRC, TRACE_KERNELS_LIB, force, verbose)
+
+
+def build_device_query_batch_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_query_batch_kernels.cu: the test queriers of DeviceView::query (overlap, nearest, containment,
+    Barnes-Hut) and the same queriers one thread per query."""
+    return _build_test_kernels(QUERY_BATCH_KERNELS_SRC, QUERY_BATCH_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

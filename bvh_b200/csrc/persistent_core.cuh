@@ -8,8 +8,8 @@
 // afford.  A round is then a bounded inner-node phase, a reconvergence point and one leaf per lane.
 //
 // What a ray is, where it comes from, what a leaf does and where a finished ray goes belong to the kernel: the library's
-// triangle kernels (traverse.cu) and DeviceView::trace over the caller's own leaf (include/bvh/v2/cuda/intersect.cuh)
-// pass them in as callables, so both run the same rounds.
+// triangle kernels (traverse.cu), DeviceView::trace over the caller's own leaf and DeviceView::query over the caller's
+// own node test (include/bvh/v2/cuda/intersect.cuh) pass them in as callables, so all of them run the same rounds.
 #pragma once
 
 #include <cstdint>

@@ -74,6 +74,15 @@ inline TracePlan plan_trace(const TraceRequest& q) {
     return p;
 }
 
+// The scheduling of DeviceView::query (include/bvh/v2/cuda/intersect.cuh): node-test queries on the persistent
+// scheduler, with the settings every kernel but the binary closest-hit one has (8 / 8).  Untuned: nobody has measured
+// node-test queries on the H100 with other values.
+struct QueryPlan {
+    uint32_t refill_min;            // idle lanes a warp waits for before it draws new queries
+    uint32_t inner_budget;          // node steps per lane and round
+};
+inline QueryPlan plan_query() { return QueryPlan { 8u, 8u }; }
+
 // The default length of a persistent warp's private run of consecutive rays (Tunables::chunk_rays, the switch
 // "chunk_rays"), and the default rounding of the traversal stack's entries (Tunables::stack_round).
 constexpr uint32_t kDefaultRunRays = 64;

@@ -10,7 +10,8 @@
 // splits it into an inner phase and a leaf phase, traverse.cu), the host emulation compiled by
 // g++ for the CPU tests (tests/host_emul.cpp) and, through traverse_top_down with the caller's leaf,
 // the device traversal API (include/bvh/v2/cuda/intersect.cuh).  traverse_nodes is the same stack machine with the
-// caller's node test instead of the ray's (DeviceView::traverse_top_down).
+// caller's node test instead of the ray's (DeviceView::traverse_top_down); its step, node_step, is also the inner step
+// of DeviceView::query's persistent kernel.
 #pragma once
 
 #include "core.cuh"
@@ -264,6 +265,28 @@ BVH_HD decltype(auto) node_test(NodeFn& node_fn, const Node& left, const Node& r
         return node_fn(left, right);
 }
 
+// One step of traverse_nodes: the sibling pair below `top` (an inner node) in one load_pair, register copies of the two
+// children handed to the caller's node test, and the reference's decision (descend): `top` becomes the next node to
+// visit, or kTraversalDone when both children were missed and the stack is empty.  DeviceView::query's kernel takes the
+// same step.
+template <typename T, typename Stack, typename NodeFn>
+BVH_HD void node_step(const DevNode<T>* __restrict__ nodes, typename Real<T>::UInt& top, Stack& stack, NodeFn& node_fn) {
+    using U = typename Real<T>::UInt;
+    // device slot = reference index + 1, the same offset arithmetic as inner_step
+    const DevNode<T>* p = reinterpret_cast<const DevNode<T>*>(reinterpret_cast<const unsigned char*>(nodes + 1) +
+                                                              (size_t)top * (sizeof(DevNode<T>) >> kPrimCountBits));
+    NodePair<T> pair;
+    load_pair(p, pair);
+    DevNode<T> left, right;
+    for (int k = 0; k < 6; ++k) { left.bounds[k] = pair.lb[k]; right.bounds[k] = pair.rb[k]; }
+    left.index = pair.li; right.index = pair.ri;
+    left.pad = right.pad = 0;
+    const auto [hit_left, hit_right, should_swap] = node_test(node_fn, static_cast<const DevNode<T>&>(left),
+                                                              static_cast<const DevNode<T>&>(right), index_first(top));
+    descend<U>(static_cast<bool>(hit_left), static_cast<bool>(hit_right), static_cast<bool>(should_swap),
+               pair.li, pair.ri, top, stack);
+}
+
 // Bvh::traverse_top_down with the caller's node test (reference bvh.h:124-157), for queries other than rays: box
 // overlap, point location, nearest-neighbour searches.  The traversal starts at the node index `start` with an empty
 // stack.
@@ -283,21 +306,7 @@ BVH_HD void traverse_nodes(const DevNode<T>* __restrict__ nodes, typename Real<T
     using U = typename Real<T>::UInt;
     U top = start;
     for (;;) {
-        while (index_count(top) == 0) {
-            // device slot = reference index + 1, the same offset arithmetic as inner_step
-            const DevNode<T>* p = reinterpret_cast<const DevNode<T>*>(reinterpret_cast<const unsigned char*>(nodes + 1) +
-                                                                      (size_t)top * (sizeof(DevNode<T>) >> kPrimCountBits));
-            NodePair<T> pair;
-            load_pair(p, pair);
-            DevNode<T> left, right;
-            for (int k = 0; k < 6; ++k) { left.bounds[k] = pair.lb[k]; right.bounds[k] = pair.rb[k]; }
-            left.index = pair.li; right.index = pair.ri;
-            left.pad = right.pad = 0;
-            const auto [hit_left, hit_right, should_swap] = node_test(node_fn, static_cast<const DevNode<T>&>(left),
-                                                                      static_cast<const DevNode<T>&>(right), index_first(top));
-            descend<U>(static_cast<bool>(hit_left), static_cast<bool>(hit_right), static_cast<bool>(should_swap),
-                       pair.li, pair.ri, top, stack);
-        }
+        while (index_count(top) == 0) node_step<T>(nodes, top, stack, node_fn);
         if (top == kTraversalDone<U>) break;
         const U first = index_first(top);
         const bool was_hit = static_cast<bool>(leaf_fn(first, first + (U)index_count(top)));

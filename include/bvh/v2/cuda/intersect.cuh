@@ -219,6 +219,55 @@
 //     };
 //     view.trace<false, false>(n, SphereTracer { d_rays, d_spheres, view.prim_ids, d_hit_ids }, workspace, bytes, stream);
 //
+// Whole batches of queries: view.query<IsAnyHit>(n, querier, workspace, workspace_bytes[, stream]) is the batch form of
+// traverse_top_down, on the same scheduler as trace: queries 0 .. n-1 with the caller's node test (box overlap, nearest
+// neighbour, point location, Barnes-Hut), in runs per warp, idle lanes refilled together, a shared-memory stack sized
+// from the tree's depth.  The querier is a plain struct copied to the kernel by value, with a Payload type (per-query
+// state, kept in registers) and four __device__ (or __host__ __device__) functions:
+//     void start(size_t i, Payload& p) const;                                  // query i of the batch; sets up p
+//     auto node(Payload& p, const Node& left, const Node& right) const;         // or (..., size_t left_index)
+//     bool leaf(Payload& p, size_t begin, size_t end) const;                   // BVH-order primitive range
+//     void finish(size_t i, const Payload& p) const;                           // query i is done
+//   * for every i in [0, n), start is called once, then exactly the node and leaf calls that
+//     traverse_top_down<IsAnyHit>(root_index(), stack, leaf', node') makes for that query, with the same arguments in
+//     the same order (leaf' and node' are leaf and node bound to the query's payload), then finish once.  A root that is
+//     a leaf gets one leaf call and no node call;
+//   * node returns what traverse_top_down's node function returns: anything that unpacks into (hit_left, hit_right,
+//     should_swap).  Node is View::Node.  The three-argument form receives the left child's reference index, so that it
+//     can read data written per node by traverse_bottom_up;
+//   * with IsAnyHit a true return from leaf ends the query;
+//   * queries are drawn in index order, in runs per warp, so neighbouring indices share node fetches.  No ordering holds
+//     between different queries.  The functions run on a subset of a warp's lanes: they must not use __syncthreads or
+//     full-mask warp collectives.  There is no watchdog;
+//   * the call is stream-ordered on `stream` (the handle's by default), does not synchronise the host, and sets and
+//     restores the current device.  n == 0 launches nothing.  Scheduling uses plan_query() (trace_plan.h); there is
+//     nothing to set;
+//   * workspace: view.query_workspace_bytes() bytes of device memory, as for trace.  A smaller workspace, or a tree too
+//     deep for the 200 KB shared-memory stack (float: depth > 398), throws std::length_error; a failed launch throws
+//     std::runtime_error;
+//   * compiled as plain host C++, query runs the queries serially: start, traverse_top_down with a host stack, finish.
+// The kernel is bvh::v2::cuda::device_view_query_kernel<T, IsAnyHit, Querier>, with trace's launch bounds, block size,
+// stack and run length.  Counting the primitive boxes that overlap each query box (Pick and overlaps as above):
+//
+//     struct OverlapCounter {
+//         struct Payload { bvh_bbox3f q; uint32_t count; };
+//         const bvh_bbox3f* queries; const bvh_bbox3f* boxes; const uint32_t* prim_ids; uint32_t* counts;
+//         __device__ void start(size_t i, Payload& p) const { p.q = queries[i]; p.count = 0; }
+//         __device__ Pick node(Payload& p, const View::Node& l, const View::Node& r) const {
+//             return Pick { overlaps(l.bounds, p.q), overlaps(r.bounds, p.q), false };
+//         }
+//         __device__ bool leaf(Payload& p, size_t begin, size_t end) const {
+//             for (size_t k = begin; k < end; ++k) {
+//                 const bvh_bbox3f b = boxes[prim_ids[k]];
+//                 const float f[6] = { b.min.x, b.max.x, b.min.y, b.max.y, b.min.z, b.max.z };
+//                 p.count += overlaps(f, p.q);
+//             }
+//             return false;
+//         }
+//         __device__ void finish(size_t i, const Payload& p) const { counts[i] = p.count; }
+//     };
+//     view.query<false>(n, OverlapCounter { d_queries, d_boxes, view.prim_ids, d_counts }, workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -233,6 +282,8 @@
 #include <cstdint>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "persistent_core.cuh"
@@ -269,6 +320,23 @@ template <typename U> struct VectorStack {
         elems.pop_back();
         return true;
     }
+};
+// A querier's node function bound to one query's payload, as traverse_nodes calls a node test: the three-argument form
+// when the querier has node(payload, left, right, left_index), the two-argument one otherwise.
+template <typename Querier, typename Payload, typename Node, typename = void> struct TakesLeftIndex : std::false_type {};
+template <typename Querier, typename Payload, typename Node>
+struct TakesLeftIndex<Querier, Payload, Node, std::void_t<decltype(std::declval<const Querier&>().node(
+    std::declval<Payload&>(), std::declval<const Node&>(), std::declval<const Node&>(), size_t(0)))>> : std::true_type {};
+template <typename Querier, typename Payload, typename Node, bool = TakesLeftIndex<Querier, Payload, Node>::value>
+struct BoundNode {
+    const Querier& q;
+    Payload& p;
+    BVH_HD decltype(auto) operator()(const Node& l, const Node& r) const { return q.node(p, l, r); }
+};
+template <typename Querier, typename Payload, typename Node> struct BoundNode<Querier, Payload, Node, true> {
+    const Querier& q;
+    Payload& p;
+    BVH_HD decltype(auto) operator()(const Node& l, const Node& r, size_t left) const { return q.node(p, l, r, left); }
 };
 }
 
@@ -364,6 +432,79 @@ device_view_trace_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned
         }
     };
     bvhb200::run_rounds<false>(run, has_ray, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
+                               [] {});
+}
+
+// The kernel of DeviceView::query: the same scheduler, launch settings and stack as device_view_trace_kernel, over the
+// caller's querier.  A lane draws query i through querier.start, descends with traverse_nodes' step (node_step) and the
+// querier's node test, hands its leaf to querier.leaf and retires the query through querier.finish.
+template <typename T, bool IsAnyHit, typename Querier>
+__global__ void __launch_bounds__(bvhb200::kTraceBlock, sizeof(T) == 4 ? BVH_TRACE_BLOCKS : 4)
+device_view_query_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned long long n, unsigned long long* cursor,
+                         uint32_t run_rays, uint32_t refill_min, uint32_t inner_budget, Querier querier) {
+    using U = typename bvhb200::Real<T>::UInt;
+    using Payload = typename Querier::Payload;
+    extern __shared__ __align__(128) unsigned char device_view_query_smem[];
+    constexpr unsigned kFull = 0xFFFFFFFFu;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    bvhb200::SmemStack<U> stack { reinterpret_cast<U*>(device_view_query_smem) + threadIdx.x, bvhb200::kTraceBlock, 0 };
+    const U root_index = nodes[1].index;
+
+    bvhb200::RunCursor run;
+    bool has_query = false;
+    unsigned long long index = 0;
+    Payload payload;
+    detail::BoundNode<Querier, Payload, bvhb200::DevNode<T>> node_fn { querier, payload };
+    U top = 0;
+    auto retire = [&] {
+        querier.finish(static_cast<size_t>(index), static_cast<const Payload&>(payload));
+        has_query = false;
+    };
+
+    // one draw: the idle lanes take the next queries of the warp's run, claiming a new run when it is used up
+    auto draw = [&] (unsigned idle, unsigned rank) {
+        if (run.pos == run.end) {
+            const unsigned long long first = bvhb200::claim_run(cursor, run_rays, lane, kFull);
+            if (first >= n) { run.exhausted = true; return false; }
+            run.pos = first;
+            run.end = first + run_rays < n ? first + run_rays : n;
+        }
+        const unsigned avail = (unsigned)(run.end - run.pos), want = __popc(idle);
+        const unsigned take = want < avail ? want : avail;
+        if (!has_query && rank < take) {
+            index = run.pos + rank;
+            querier.start(static_cast<size_t>(index), payload);
+            top = root_index;
+            stack.clear();
+            has_query = true;
+        }
+        run.pos += take;
+        return true;
+    };
+
+    // inner phase: node steps until this lane holds a leaf, its query is finished, or the step budget of this round is spent
+    auto inner = [&] {
+        if (has_query) {
+            uint32_t budget = inner_budget;
+            while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone ends it too)
+                --budget;
+                bvhb200::node_step<T>(nodes, top, stack, node_fn);
+            }
+            if (top == bvhb200::kTraversalDone<U>) retire();
+        }
+    };
+
+    // leaf phase: the caller's leaf; the query ends on an any-hit hit or an empty stack
+    auto leaf = [&] {
+        if (has_query && bvhb200::index_count(top) != 0) {
+            const U first = bvhb200::index_first(top);
+            const bool hit = static_cast<bool>(querier.leaf(payload, static_cast<size_t>(first),
+                                                            static_cast<size_t>(first + (U)bvhb200::index_count(top))));
+            if ((IsAnyHit && hit) || !stack.try_pop(top)) retire();
+        }
+    };
+    bvhb200::run_rounds<false>(run, has_query, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
                                [] {});
 }
 #endif
@@ -507,47 +648,18 @@ template <typename T> struct DeviceView {
     // `on_stream` is a cudaStream_t (unused by the host pass)
     template <bool IsAnyHit, bool IsRobust, typename Tracer>
     void trace(size_t n, const Tracer& tracer, void* workspace, size_t workspace_bytes, void* on_stream) const {
-        const size_t need = trace_workspace_bytes();
-        if (workspace_bytes < need || !workspace)
-            throw std::length_error("bvh::v2::cuda::DeviceView::trace: a workspace of " + std::to_string(workspace ? workspace_bytes : 0) +
-                                    " bytes is too small (" + std::to_string(need) + " bytes)");
-        // the batched kernels' shared-memory stack, sized and bounded as bvhNN_intersect_rays sizes and bounds it
-        const size_t smem = (size_t)bvhb200::stack_entries(static_cast<uint32_t>(depth), bvhb200::kDefaultStackRound) *
-                            bvhb200::kTraceBlock * sizeof(Index);
-        if (smem > kMaxTraceSmem)
-            throw std::length_error("bvh::v2::cuda::DeviceView::trace: a tree of depth " + std::to_string(depth) + " needs " +
-                                    std::to_string(smem) + " bytes of shared-memory stack per block, more than " +
-                                    std::to_string(kMaxTraceSmem));
-        if (n == 0) return;
+        // the library's scheduling of a persistent closest-hit or any-hit batch, with its default settings
+        bvhb200::TraceRequest request {};
+        request.flags = bvhb200::kTraceNoTma | (IsAnyHit ? bvhb200::kTraceAnyHit : 0u) | (IsRobust ? bvhb200::kTraceRobust : 0u);
+        request.is_float = sizeof(T) == 4;
+        request.n = n;
+        const bvhb200::TracePlan plan = bvhb200::plan_trace(request);
 #if defined(__CUDACC__)
-        cudaStream_t s = static_cast<cudaStream_t>(on_stream);
-        int previous = 0;
-        check(cudaGetDevice(&previous), "cudaGetDevice", "trace");
-        if (previous != device) check(cudaSetDevice(device), "cudaSetDevice", "trace");
-        void (*kernel)(const Node*, unsigned long long, unsigned long long*, uint32_t, uint32_t, uint32_t, Tracer) =
-            device_view_trace_kernel<T, IsAnyHit, IsRobust, Tracer>;
-        int sm_count = 0, per_sm = 0;
-        cudaError_t e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device);
-        if (e == cudaSuccess && smem > 48 * 1024) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, bvhb200::kTraceBlock, smem);
-        if (e == cudaSuccess) e = cudaMemsetAsync(workspace, 0, need, s);
-        if (e == cudaSuccess) {
-            // the library's scheduling of a persistent closest-hit or any-hit batch, with its default settings
-            bvhb200::TraceRequest request {};
-            request.flags = bvhb200::kTraceNoTma | (IsAnyHit ? bvhb200::kTraceAnyHit : 0u) | (IsRobust ? bvhb200::kTraceRobust : 0u);
-            request.is_float = sizeof(T) == 4;
-            request.n = n;
-            const bvhb200::TracePlan plan = bvhb200::plan_trace(request);
-            const uint32_t run_rays = bvhb200::persistent_run_rays(bvhb200::kDefaultRunRays, n, sm_count);
-            const unsigned long long grid = bvhb200::persistent_grid(sm_count, per_sm, n, 32, bvhb200::kTraceBlock / 32);
-            kernel<<<(unsigned)grid, bvhb200::kTraceBlock, smem, s>>>(nodes, n, static_cast<unsigned long long*>(workspace), run_rays,
-                                                                     plan.refill_min, plan.inner_budget, tracer);
-            e = cudaGetLastError();
-        }
-        if (previous != device) cudaSetDevice(previous);
-        check(e, "launch", "trace");
+        run_batch("trace", device_view_trace_kernel<T, IsAnyHit, IsRobust, Tracer>, tracer, n, plan.refill_min, plan.inner_budget,
+                  workspace, workspace_bytes, on_stream);
 #else
-        (void)on_stream;
+        (void)on_stream; (void)plan;
+        batch_stack_bytes("trace", workspace, workspace_bytes);
         using Payload = typename Tracer::Payload;
         for (size_t i = 0; i < n; ++i) {
             Payload payload;
@@ -569,6 +681,38 @@ template <typename T> struct DeviceView {
 #endif
     }
 
+    // A whole batch of node-test queries on the same scheduler, with the caller's querier: see "Whole batches of
+    // queries" at the top of this file.  The workspace is the warps' run cursor, as trace's.
+    BVH_HD size_t query_workspace_bytes() const { return sizeof(unsigned long long); }
+
+    template <bool IsAnyHit, typename Querier>
+    void query(size_t n, const Querier& querier, void* workspace, size_t workspace_bytes) const {
+        query<IsAnyHit>(n, querier, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsAnyHit, typename Querier>
+    void query(size_t n, const Querier& querier, void* workspace, size_t workspace_bytes, void* on_stream) const {
+        const bvhb200::QueryPlan plan = bvhb200::plan_query();
+#if defined(__CUDACC__)
+        run_batch("query", device_view_query_kernel<T, IsAnyHit, Querier>, querier, n, plan.refill_min, plan.inner_budget,
+                  workspace, workspace_bytes, on_stream);
+#else
+        (void)on_stream; (void)plan;
+        batch_stack_bytes("query", workspace, workspace_bytes);
+        using Payload = typename Querier::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            querier.start(i, payload);
+            detail::VectorStack<Index> stack;
+            stack.elems.reserve(stack_bound());
+            traverse_top_down<IsAnyHit>(root_index(), stack,
+                                        [&](size_t begin, size_t end) { return static_cast<bool>(querier.leaf(payload, begin, end)); },
+                                        detail::BoundNode<Querier, Payload, Node> { querier, payload });
+            querier.finish(i, static_cast<const Payload&>(payload));
+        }
+#endif
+    }
+
     // PrecomputedTri::intersect (reference tri.h:55-74) on BVH-order triangle k: true, with the hit's distance and
     // barycentrics, when the ray meets it at a distance in [ray.tmin, ray.tmax].  The batched kernels' own test.
     BVH_HD bool intersect_tri(size_t k, const Ray& ray, T& t, T& u, T& v) const {
@@ -585,6 +729,52 @@ template <typename T> struct DeviceView {
 private:
     // the shared memory a persistent block may have, as bvhNN_intersect_rays bounds it
     static constexpr size_t kMaxTraceSmem = 200 * 1024;
+
+    // The checks of trace and query (`call`): the workspace, then the shared-memory stack of the batched kernels, sized
+    // and bounded as bvhNN_intersect_rays sizes and bounds it.  Returns the stack's bytes per block.
+    size_t batch_stack_bytes(const char* call, void* workspace, size_t workspace_bytes) const {
+        const std::string who = std::string("bvh::v2::cuda::DeviceView::") + call;
+        const size_t need = trace_workspace_bytes();
+        if (workspace_bytes < need || !workspace)
+            throw std::length_error(who + ": a workspace of " + std::to_string(workspace ? workspace_bytes : 0) + " bytes is too small (" +
+                                    std::to_string(need) + " bytes)");
+        const size_t smem = (size_t)bvhb200::stack_entries(static_cast<uint32_t>(depth), bvhb200::kDefaultStackRound) *
+                            bvhb200::kTraceBlock * sizeof(Index);
+        if (smem > kMaxTraceSmem)
+            throw std::length_error(who + ": a tree of depth " + std::to_string(depth) + " needs " + std::to_string(smem) +
+                                    " bytes of shared-memory stack per block, more than " + std::to_string(kMaxTraceSmem));
+        return smem;
+    }
+#if defined(__CUDACC__)
+    // The launch of trace and query: the checks, then, unless n == 0, the current device switched to the tree's, the run
+    // cursor reset, and one resident wave of `kernel` (device_view_trace_kernel or device_view_query_kernel) on
+    // `on_stream` with the run length and grid of bvhNN_intersect_rays' persistent kernel.
+    template <typename Fn>
+    void run_batch(const char* call, void (*kernel)(const Node*, unsigned long long, unsigned long long*, uint32_t, uint32_t, uint32_t, Fn),
+                   const Fn& fn, size_t n, uint32_t refill_min, uint32_t inner_budget, void* workspace, size_t workspace_bytes,
+                   void* on_stream) const {
+        const size_t smem = batch_stack_bytes(call, workspace, workspace_bytes);
+        if (n == 0) return;
+        cudaStream_t s = static_cast<cudaStream_t>(on_stream);
+        int previous = 0;
+        check(cudaGetDevice(&previous), "cudaGetDevice", call);
+        if (previous != device) check(cudaSetDevice(device), "cudaSetDevice", call);
+        int sm_count = 0, per_sm = 0;
+        cudaError_t e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device);
+        if (e == cudaSuccess && smem > 48 * 1024) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, bvhb200::kTraceBlock, smem);
+        if (e == cudaSuccess) e = cudaMemsetAsync(workspace, 0, trace_workspace_bytes(), s);
+        if (e == cudaSuccess) {
+            const uint32_t run_rays = bvhb200::persistent_run_rays(bvhb200::kDefaultRunRays, n, sm_count);
+            const unsigned long long grid = bvhb200::persistent_grid(sm_count, per_sm, n, 32, bvhb200::kTraceBlock / 32);
+            kernel<<<(unsigned)grid, bvhb200::kTraceBlock, smem, s>>>(nodes, n, static_cast<unsigned long long*>(workspace), run_rays,
+                                                                     refill_min, inner_budget, fn);
+            e = cudaGetLastError();
+        }
+        if (previous != device) cudaSetDevice(previous);
+        check(e, "launch", call);
+    }
+#endif
 #if defined(__CUDACC__)
     static void check(cudaError_t e, const char* what, const char* call = "traverse_bottom_up") {
         if (e != cudaSuccess)

@@ -12,6 +12,11 @@ Prints the card's name and power limit, then one JSON line with the median of `s
   mass_ms              the pass with subtree mass and centre of mass (MassCentre)
   barnes_hut_ms        the softened potential at every particle, theta = 0.5, through traverse_top_down with the
                        three-argument node test (Potential), one thread per particle
+  barnes_hut_query_ms  the same potential as one batch through DeviceView::query (tests/device_query_batch_kernels.cu)
+  *_bvh_order_ms       both again with the particles queried in BVH order (query i takes particle prim_ids[i])
+                       instead of their random original order
+                       Before each pair is timed, its potentials are checked equal bit for bit (barnes_hut_match,
+                       barnes_hut_bvh_order_match)
 The passes include their link kernel and workspace set-up; they run the test kernels of tests/device_bottom_up_kernels.cu
 (built by build()).
 """
@@ -155,9 +160,31 @@ def main():
     row["mass_ms"] = timed(lambda: ok(bu.bu_mass3f(h, ws.data_ptr(), nbytes.value, d_pos.data_ptr(), d_mass.data_ptr(),
                                                    node_mass.data_ptr(), node_centre.data_ptr())))
     eps2 = float((0.1 / np.cbrt(n)) ** 2)
-    row["barnes_hut_ms"] = timed(lambda: ok(bu.bu_potential3f(h, d_pos.data_ptr(), d_mass.data_ptr(), node_mass.data_ptr(),
-                                                              node_centre.data_ptr(), d_pos.data_ptr(), n, 0.25, eps2,
-                                                              phi.data_ptr(), None)))
+    dqb = C.CDLL(build_ext.build_device_query_batch_tests())
+    dqb.dqb_potential3f.argtypes = [P, P, P, P, P, P, SZ, C.c_float, C.c_float, P, P, P, SZ, P]
+    dqb.dqb_last_error.restype = C.c_char_p
+    ok(bu.bu_mass3f(h, ws.data_ptr(), nbytes.value, d_pos.data_ptr(), d_mass.data_ptr(), node_mass.data_ptr(),
+                    node_centre.data_ptr()))
+    cursor = torch.empty(8, dtype=torch.uint8, device="cuda")
+    phi_query = torch.empty(n, dtype=torch.float32, device="cuda")
+
+    def per_thread(points):
+        ok(bu.bu_potential3f(h, d_pos.data_ptr(), d_mass.data_ptr(), node_mass.data_ptr(), node_centre.data_ptr(),
+                             points.data_ptr(), n, 0.25, eps2, phi.data_ptr(), None))
+
+    def batch(points):
+        rc = dqb.dqb_potential3f(h, d_pos.data_ptr(), d_mass.data_ptr(), node_mass.data_ptr(), node_centre.data_ptr(),
+                                 points.data_ptr(), n, 0.25, eps2, phi_query.data_ptr(), None, cursor.data_ptr(), 8, None)
+        assert rc == 0, dqb.dqb_last_error()
+
+    bvh_order = torch.from_numpy(bvh.arrays()[2].astype(np.int64)).cuda()
+    for suffix, points in (("", d_pos), ("_bvh_order", d_pos[bvh_order].contiguous())):
+        per_thread(points)
+        batch(points)
+        torch.cuda.synchronize()
+        row[f"barnes_hut{suffix}_match"] = bool(torch.equal(phi.view(torch.int32), phi_query.view(torch.int32)))
+        row[f"barnes_hut{suffix}_ms"] = timed(lambda: per_thread(points))
+        row[f"barnes_hut_query{suffix}_ms"] = timed(lambda: batch(points))
     torch.cuda.synchronize()
     bounds = bvh.arrays()[0]
     row["count_box_matches_tree"] = bool((node_boxes.cpu().numpy().view(np.uint32) == bounds.view(np.uint32)).all())

@@ -11,6 +11,9 @@ Prints the card's name and power limit, then one JSON line with the median of `s
                     (`_array`) and the shared-memory stack (`_shared`); CUDA events on the handle's stream
   nearest_ms        the nearest sphere centre to each of n random points in the unit cube (nearest_kernel), both stacks;
                     CUDA events
+  overlap_ms_query, nearest_ms_query  the same two queries as batches through DeviceView::query on the persistent
+                    scheduler (tests/device_query_batch_kernels.cu); before they are timed, their outputs are checked equal
+                    to the per-thread kernels' (query_matches_per_thread)
 and the number of overlapping pairs the broad phase found (each unordered pair of distinct spheres once).  Nothing is
 written to the tree except the test kernels' build under tests/_build when it is stale.
 """
@@ -55,6 +58,9 @@ def main():
     dq.dq_overlap3f.argtypes = [P, P, P, SZ, C.c_int, P, P, P, P, P]
     dq.dq_nearest3f.argtypes = [P, P, P, SZ, C.c_int, P, P, P, P, P]
     dq.dq_last_error.restype = C.c_char_p
+    dqb = C.CDLL(build_ext.build_device_query_batch_tests())
+    dqb.dqb_query3f.argtypes = [P, C.c_int, C.c_int, C.c_int, P, P, SZ, P, P, P, P, P, P, P, SZ, P]
+    dqb.dqb_last_error.restype = C.c_char_p
     api.set_device(0)
     torch.cuda.set_device(0)
     stream = torch.cuda.current_stream()
@@ -112,6 +118,30 @@ def main():
         row[f"nearest_ms_{label}"] = event_timed(lambda: check(dq.dq_nearest3f(
             C.c_void_p(bvh.handle), d_centers.data_ptr(), points.data_ptr(), n, stack, ids.data_ptr(), dist2.data_ptr(),
             None, None, None)))
+    # the same queries through DeviceView::query: outputs checked equal to the per-thread kernels' first, then timed
+    ws = torch.empty(8, dtype=torch.uint8, device="cuda")
+    idsums = torch.zeros(n, dtype=torch.int64, device="cuda")
+
+    def batch(kind, prims, queries, r0, r1):
+        rc = dqb.dqb_query3f(C.c_void_p(bvh.handle), kind, 0, 0, prims.data_ptr(), queries.data_ptr(), n, r0.data_ptr(),
+                             r1.data_ptr(), None, None, None, None, ws.data_ptr(), 8, None)
+        if rc:
+            raise RuntimeError(dqb.dqb_last_error().decode())
+
+    check(dq.dq_overlap3f(C.c_void_p(bvh.handle), d_boxes.data_ptr(), d_boxes.data_ptr(), n, 0, counts.data_ptr(),
+                          idsums.data_ptr(), None, None, None))
+    check(dq.dq_nearest3f(C.c_void_p(bvh.handle), d_centers.data_ptr(), points.data_ptr(), n, 0, ids.data_ptr(),
+                          dist2.data_ptr(), None, None, None))
+    want = [t.clone() for t in (counts, idsums, ids, dist2)]
+    q_counts, q_idsums, q_ids, q_dist2 = (torch.zeros_like(t) for t in want)
+    batch(0, d_boxes, d_boxes, q_counts, q_idsums)
+    batch(1, d_centers, points, q_ids, q_dist2)
+    torch.cuda.synchronize()
+    row["query_matches_per_thread"] = all(bool(torch.equal(a, b)) for a, b in
+                                          zip(want[:3] + [want[3].view(torch.int32)],
+                                              [q_counts, q_idsums, q_ids, q_dist2.view(torch.int32)]))
+    row["overlap_ms_query"] = event_timed(lambda: batch(0, d_boxes, d_boxes, q_counts, q_idsums))
+    row["nearest_ms_query"] = event_timed(lambda: batch(1, d_centers, points, q_ids, q_dist2))
     row["depth"] = bvh.depth
     row["card"], row["power_limit"] = name, power
     print(json.dumps(row), flush=True)
