@@ -72,6 +72,8 @@ TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_trace_kernels.cu")
 TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_trace_kernels.so")
 QUERY_BATCH_KERNELS_SRC = os.path.join(ROOT, "tests", "device_query_batch_kernels.cu")
 QUERY_BATCH_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_query_batch_kernels.so")
+TRIANGLE_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_triangle_trace_kernels.cu")
+TRIANGLE_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_triangle_trace_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -126,6 +128,12 @@ def build_device_query_batch_tests(force: bool = False, verbose: bool = False) -
     """tests/device_query_batch_kernels.cu: the test queriers of DeviceView::query (overlap, nearest, containment,
     Barnes-Hut) and the same queriers one thread per query."""
     return _build_test_kernels(QUERY_BATCH_KERNELS_SRC, QUERY_BATCH_KERNELS_LIB, force, verbose)
+
+
+def build_device_triangle_trace_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_triangle_trace_kernels.cu: the test shaders of DeviceView::trace_triangles (recording filters, the
+    plain array shader, an in-kernel camera) and the same filters one thread per ray."""
+    return _build_test_kernels(TRIANGLE_TRACE_KERNELS_SRC, TRIANGLE_TRACE_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

@@ -280,14 +280,21 @@ template <typename T> struct HitState {
     T t, u, v;
 };
 
+// tri_test's default filter: every candidate hit counts.
+struct AcceptAll {
+    template <typename T> BVH_HD bool operator()(uint32_t, T, T, T) const { return true; }
+};
+
 // reference tri.h:55-74 with the caller's leaf convention (benchmark.cpp:281-292).  Returns true
 // when the triangle was accepted as the new closest hit (and tmax was shrunk).
 //   kLowestId = false: reference example semantics, `t <= tmax` so the LAST visited of equal-t hits wins
 //   kLowestId = true : canonical tree-independent rule, accept iff t < best || (t == best && id < best id)
 //                      with ids being ORIGINAL primitive ids (prim_ids[slot]); a miss has id UINT_MAX
-template <typename T>
+// accept(slot, t, u, v) is the caller's filter (DeviceView::trace_triangles): called for a triangle that passes the test,
+// the interval and the tie rule, before anything is updated; false drops the hit.
+template <typename T, typename Accept = AcceptAll>
 BVH_HD bool tri_test(const DevTri<T>& tri, uint32_t slot, const uint32_t* __restrict__ prim_ids,
-                     bool kLowestId, RayCtx<T>& r, HitState<T>& hit) {
+                     bool kLowestId, RayCtx<T>& r, HitState<T>& hit, Accept&& accept = {}) {
     using R = Real<T>;
     const T tolerance = R::neg(R::eps());
     T c[3] = { R::sub(tri.p0[0], r.org[0]), R::sub(tri.p0[1], r.org[1]), R::sub(tri.p0[2], r.org[2]) };
@@ -305,6 +312,7 @@ BVH_HD bool tri_test(const DevTri<T>& tri, uint32_t slot, const uint32_t* __rest
                     if (!(prim_ids[slot] < prim_ids[hit.slot])) return false;
                 }
             }
+            if (!accept(slot, t, u, v)) return false;
             r.tmax = t;
             hit.slot = slot; hit.t = t; hit.u = u; hit.v = v;
             return true;

@@ -75,17 +75,7 @@ __device__ __forceinline__ void multimem_store_v4(void* p, uint4 v) {
                  :: "l"(p), "f"(__uint_as_float(v.x)), "f"(__uint_as_float(v.y)), "f"(__uint_as_float(v.z)), "f"(__uint_as_float(v.w)) : "memory");
 }
 
-// A miss reports id = all ones (BVH_INVALID_PRIM_ID), t = the ray's tmax, u = v = 0.
-template <typename T>
-__device__ __forceinline__ DevHit<T> make_record(const HitState<T>& h, T tmax, const uint32_t* __restrict__ prim_ids) {
-    DevHit<T> rec;
-    const bool was_hit = h.slot != kInvalidId;
-    rec.prim_id = was_hit ? (decltype(rec.prim_id))prim_ids[h.slot] : (decltype(rec.prim_id))~(decltype(rec.prim_id))0;
-    rec.t = was_hit ? h.t : tmax;
-    rec.u = was_hit ? h.u : (T)0;
-    rec.v = was_hit ? h.v : (T)0;
-    return rec;
-}
+// (a finished ray's record: make_record, traverse_core.cuh)
 
 // One record to every sink with one store per sink (16-byte pieces).
 template <typename T>

@@ -316,15 +316,42 @@ BVH_HD void traverse_nodes(const DevNode<T>* __restrict__ nodes, typename Real<T
 }
 
 // The triangles [first, first + count) of a leaf (benchmark.cpp:281-292).  stats (nullable): [1] leaves, [2] triangle tests.
-template <typename T>
+// accept: tri_test's filter, called with the slot, t, u and v of every candidate that would become the closest hit.  With a
+// filter of the caller's the loop is not unrolled: one copy of the caller's code, and one triangle's registers live at a
+// time (DeviceView::trace_triangles' float kernel then fits its 56 registers without spills; DESIGN.md §6).
+template <typename T, typename Accept = AcceptAll>
 BVH_HD void leaf_range(const DevTri<T>* __restrict__ tris, const uint32_t* __restrict__ prim_ids, bool lowest_id,
-                       uint32_t first, uint32_t count, RayCtx<T>& r, HitState<T>& hit, uint32_t* stats) {
+                       uint32_t first, uint32_t count, RayCtx<T>& r, HitState<T>& hit, uint32_t* stats, Accept&& accept = {}) {
     if (stats) { stats[1] += 1; stats[2] += count; }
-    for (uint32_t i = first; i < first + count; ++i) {
-        DevTri<T> tri;
-        load_tri(tris + i, tri);
-        tri_test<T>(tri, i, prim_ids, lowest_id, r, hit);
+    if constexpr (std::is_same_v<std::decay_t<Accept>, AcceptAll>) {
+        for (uint32_t i = first; i < first + count; ++i) {
+            DevTri<T> tri;
+            load_tri(tris + i, tri);
+            tri_test<T>(tri, i, prim_ids, lowest_id, r, hit);
+        }
+    } else {
+#if defined(__CUDA_ARCH__)
+        #pragma unroll 1
+#endif
+        for (uint32_t i = first; i < first + count; ++i) {
+            DevTri<T> tri;
+            load_tri(tris + i, tri);
+            tri_test<T>(tri, i, prim_ids, lowest_id, r, hit, accept);
+        }
     }
+}
+
+// The hit record of a finished ray (bvh_hit3f / bvh_hit3d): its closest hit's original id, t, u and v; a miss reports
+// id = all ones (BVH_INVALID_PRIM_ID), t = the ray's tmax, u = v = 0.
+template <typename T>
+BVH_HD DevHit<T> make_record(const HitState<T>& h, T tmax, const uint32_t* __restrict__ prim_ids) {
+    DevHit<T> rec;
+    const bool was_hit = h.slot != kInvalidId;
+    rec.prim_id = was_hit ? (decltype(rec.prim_id))prim_ids[h.slot] : (decltype(rec.prim_id))~(decltype(rec.prim_id))0;
+    rec.t = was_hit ? h.t : tmax;
+    rec.u = was_hit ? h.u : (T)0;
+    rec.v = was_hit ? h.v : (T)0;
+    return rec;
 }
 
 // Leaf processing for the leaf index `top`.

@@ -268,6 +268,47 @@
 //     };
 //     view.query<false>(n, OverlapCounter { d_queries, d_boxes, view.prim_ids, d_counts }, workspace, bytes, stream);
 //
+// Whole batches of triangle rays: view.trace_triangles<IsAnyHit, IsRobust, TieLastVisited = false>(n, shader, workspace,
+// workspace_bytes[, stream]) runs the library's own triangle traversal (the inner step, leaf and record of
+// bvhNN_intersect_rays' persistent kernel) on the scheduler trace uses, with the caller's ray source, hit filter and hit
+// sink: what OptiX calls raygen, any-hit and closest-hit programs, reduced to the library's semantics.  The view must have
+// triangles (a tree from bvhNN_build_triangles or with bvhNN_set_triangles).  The shader is a plain struct copied to the
+// kernel by value, with a Payload type (per-ray state, kept in registers) and three __device__ (or __host__ __device__)
+// functions:
+//     Ray  start(size_t i, Payload& p) const;                                  // ray i of the batch; sets up p
+//     bool accept(Payload& p, size_t prim_id, T t, T u, T v) const;             // a candidate hit; false: ignore it
+//     void finish(size_t i, const Payload& p, const Hit& hit) const;           // ray i is done; Hit is bvh_hit3f / 3d
+//   * for every i in [0, n), start is called once, then the accept calls, then finish once;
+//   * accept is called once per triangle of each leaf reached (in BVH order within the leaf, leaves in the reference's
+//     visit order) that passes PrecomputedTri::intersect with its t in [tmin, tmax] and that the tie rule would take as
+//     the new closest hit: the lowest original id at equal t, or the last visited with TieLastVisited
+//     (BVH_TIE_LAST_VISITED).  prim_id is the original id.  The accept calls of a ray are exactly those a host leaf loop
+//     running the same test, tie rule and filter makes in Bvh::intersect<IsAnyHit, IsRobust> on the same tree;
+//   * true from accept records the hit and shrinks tmax; with IsAnyHit the ray then ends after that leaf (the leaf's
+//     remaining triangles are still tested, as in the library's kernel).  false changes nothing;
+//   * finish receives the record bvhNN_intersect_rays writes: the original id, or all ones on a miss; t, or the input
+//     tmax on a miss; u and v, or 0 on a miss.  A shader whose accept returns true and whose start and finish read and
+//     write arrays reproduces bvhNN_intersect_rays(flags) bit for bit.  A ray whose interval is a NaN gets no accept call
+//     and finishes as a miss, as in the library's kernels;
+//   * ordering, the warp subset (no __syncthreads, no full-mask collectives), no watchdog, streams, n == 0 and the host
+//     build are those of trace.  workspace: view.trace_workspace_bytes() bytes (the run cursor).  A smaller workspace or a
+//     tree too deep for the 200 KB shared-memory stack throws std::length_error, a view without triangles
+//     std::invalid_argument, a failed launch std::runtime_error.  Compiled as plain host C++, the rays run serially.
+// The kernel is bvh::v2::cuda::device_view_triangle_kernel<T, IsAnyHit, IsRobust, TieLastVisited, Shader>, with trace's
+// launch bounds, block and stack and the scheduling of bvhNN_intersect_rays' persistent kernel (14 / 4 for closest-hit
+// rays).  Under the float bounds (56 registers) an empty payload does not spill; every word of payload competes with the
+// traversal's own state, so keep it to a few words.  Shadow rays that leave a surface skip the triangle they start on
+// (self-intersection):
+//
+//     struct ShadowShader {
+//         struct Payload { uint32_t origin; };
+//         const bvh_ray3f* rays; const uint32_t* origin_ids; uint8_t* lit;   // origin_ids: the triangle each ray leaves
+//         __device__ bvh_ray3f start(size_t i, Payload& p) const { p.origin = origin_ids[i]; return rays[i]; }
+//         __device__ bool accept(Payload& p, size_t prim_id, float, float, float) const { return prim_id != p.origin; }
+//         __device__ void finish(size_t i, const Payload&, const bvh_hit3f& hit) const { lit[i] = hit.prim_id == UINT32_MAX; }
+//     };
+//     view.trace_triangles<true, false>(n, ShadowShader { d_rays, d_origins, d_lit }, workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -295,8 +336,8 @@ namespace bvh::v2::cuda {
 
 namespace detail {
 template <typename T> struct ViewTypes;
-template <> struct ViewTypes<float>  { using CView = bvh_device_view3f; using Ray = bvh_ray3f; };
-template <> struct ViewTypes<double> { using CView = bvh_device_view3d; using Ray = bvh_ray3d; };
+template <> struct ViewTypes<float>  { using CView = bvh_device_view3f; using Ray = bvh_ray3f; using Hit = bvh_hit3f; };
+template <> struct ViewTypes<double> { using CView = bvh_device_view3d; using Ray = bvh_ray3d; using Hit = bvh_hit3d; };
 struct NoInnerFn { template <typename I> BVH_HD void operator()(I) const {} };
 template <typename T, typename Ray> BVH_HD void load_ray(const Ray& ray, bvhb200::RayCtx<T>& r) {
     r.org[0] = ray.org.x; r.org[1] = ray.org.y; r.org[2] = ray.org.z;
@@ -338,6 +379,28 @@ template <typename Querier, typename Payload, typename Node> struct BoundNode<Qu
     Payload& p;
     BVH_HD decltype(auto) operator()(const Node& l, const Node& r, size_t left) const { return q.node(p, l, r, left); }
 };
+// The library's hit record as the C ABI reports it
+template <typename T> BVH_HD typename ViewTypes<T>::Hit make_hit(const bvhb200::DevHit<T>& rec) {
+    typename ViewTypes<T>::Hit hit;
+    hit.prim_id = rec.prim_id; hit.t = rec.t; hit.u = rec.u; hit.v = rec.v;
+    return hit;
+}
+// What the kernel of DeviceView::trace_triangles reads besides the nodes: the caller's shader and the tree's triangles.
+template <typename T, typename Shader> struct TriangleShader {
+    Shader shader;
+    const bvhb200::DevTri<T>* tris;     // BVH order
+    const uint32_t* prim_ids;
+};
+// The triangle leaf of DeviceView::trace_triangles (both builds): the library's leaf_range over [first, first + count)
+// with the shader's accept as tri_test's filter, which receives the original id.
+template <typename T, bool TieLastVisited, typename Shader, typename Payload>
+BVH_HD void shader_leaf(const TriangleShader<T, Shader>& ts, Payload& payload, uint32_t first, uint32_t count,
+                        bvhb200::RayCtx<T>& r, bvhb200::HitState<T>& hit) {
+    bvhb200::leaf_range<T>(ts.tris, ts.prim_ids, !TieLastVisited, first, count, r, hit, nullptr,
+                           [&](uint32_t slot, T t, T u, T v) {
+                               return static_cast<bool>(ts.shader.accept(payload, static_cast<size_t>(ts.prim_ids[slot]), t, u, v));
+                           });
+}
 }
 
 #if defined(__CUDACC__)
@@ -353,6 +416,27 @@ __global__ void bottom_up_climb_kernel(const bvhb200::DevNode<T>* nodes, size_t 
                                        int* __restrict__ flags, LeafFn leaf_fn, InnerFn inner_fn) {
     const size_t i = 1 + blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i < slots) bvhb200::climb_from_leaf<T>(nodes, i, parent, flags, leaf_fn, inner_fn);
+}
+
+namespace detail {
+// One draw of the DeviceView batch kernels: the idle lanes take the next indices of the warp's run, claiming a new run of
+// `run_rays` from `cursor` when it is used up.  begin(i) starts index i on each lane that is not `busy` and takes one.
+// False, with the run exhausted, when the batch has none left.
+template <typename Begin>
+__device__ __forceinline__ bool draw_run(bvhb200::RunCursor& run, unsigned long long* cursor, unsigned long long n, uint32_t run_rays,
+                                         unsigned lane, bool busy, unsigned idle, unsigned rank, Begin&& begin) {
+    if (run.pos == run.end) {
+        const unsigned long long first = bvhb200::claim_run(cursor, run_rays, lane, 0xFFFFFFFFu);
+        if (first >= n) { run.exhausted = true; return false; }
+        run.pos = first;
+        run.end = first + run_rays < n ? first + run_rays : n;
+    }
+    const unsigned avail = (unsigned)(run.end - run.pos), want = __popc(idle);
+    const unsigned take = want < avail ? want : avail;
+    if (!busy && rank < take) begin(run.pos + rank);
+    run.pos += take;
+    return true;
+}
 }
 
 // The kernel of DeviceView::trace: the library's persistent scheduler (persistent_core.cuh) over the caller's tracer.
@@ -383,26 +467,16 @@ device_view_trace_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned
         has_ray = false;
     };
 
-    // one draw: the idle lanes take the next rays of the warp's run, claiming a new run when it is used up
+    // one draw: the idle lanes take the next rays of the warp's run
     auto draw = [&] (unsigned idle, unsigned rank) {
-        if (run.pos == run.end) {
-            const unsigned long long first = bvhb200::claim_run(cursor, run_rays, lane, kFull);
-            if (first >= n) { run.exhausted = true; return false; }
-            run.pos = first;
-            run.end = first + run_rays < n ? first + run_rays : n;
-        }
-        const unsigned avail = (unsigned)(run.end - run.pos), want = __popc(idle);
-        const unsigned take = want < avail ? want : avail;
-        if (!has_ray && rank < take) {
-            index = run.pos + rank;
+        return detail::draw_run(run, cursor, n, run_rays, lane, has_ray, idle, rank, [&] (unsigned long long i) {
+            index = i;
             detail::load_ray<T>(tracer.start(static_cast<size_t>(index), payload), r);
             bvhb200::ray_prologue<T, IsRobust>(r);
             top = root_index;
             stack.clear();
             has_ray = true;
-        }
-        run.pos += take;
-        return true;
+        });
     };
 
     // inner phase: descend until this lane holds a leaf, its ray is finished, or the step budget of this round is spent
@@ -462,25 +536,15 @@ device_view_query_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned
         has_query = false;
     };
 
-    // one draw: the idle lanes take the next queries of the warp's run, claiming a new run when it is used up
+    // one draw: the idle lanes take the next queries of the warp's run
     auto draw = [&] (unsigned idle, unsigned rank) {
-        if (run.pos == run.end) {
-            const unsigned long long first = bvhb200::claim_run(cursor, run_rays, lane, kFull);
-            if (first >= n) { run.exhausted = true; return false; }
-            run.pos = first;
-            run.end = first + run_rays < n ? first + run_rays : n;
-        }
-        const unsigned avail = (unsigned)(run.end - run.pos), want = __popc(idle);
-        const unsigned take = want < avail ? want : avail;
-        if (!has_query && rank < take) {
-            index = run.pos + rank;
+        return detail::draw_run(run, cursor, n, run_rays, lane, has_query, idle, rank, [&] (unsigned long long i) {
+            index = i;
             querier.start(static_cast<size_t>(index), payload);
             top = root_index;
             stack.clear();
             has_query = true;
-        }
-        run.pos += take;
-        return true;
+        });
     };
 
     // inner phase: node steps until this lane holds a leaf, its query is finished, or the step budget of this round is spent
@@ -507,6 +571,74 @@ device_view_query_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned
     bvhb200::run_rounds<false>(run, has_query, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
                                [] {});
 }
+
+// The kernel of DeviceView::trace_triangles: the same scheduler, launch settings and stack as device_view_trace_kernel, with
+// the library's own triangle traversal.  A lane draws ray i through shader.start (a ray whose interval is a NaN retires at
+// once as a miss), descends with the library's inner step, tests its leaf's triangles against its RayCtx in registers
+// with the shader's accept as the filter, and retires the ray with the library's record through shader.finish.
+template <typename T, bool IsAnyHit, bool IsRobust, bool TieLastVisited, typename Shader>
+__global__ void __launch_bounds__(bvhb200::kTraceBlock, sizeof(T) == 4 ? BVH_TRACE_BLOCKS : 4)
+device_view_triangle_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned long long n, unsigned long long* cursor,
+                            uint32_t run_rays, uint32_t refill_min, uint32_t inner_budget, detail::TriangleShader<T, Shader> ts) {
+    using U = typename bvhb200::Real<T>::UInt;
+    using Payload = typename Shader::Payload;
+    extern __shared__ __align__(128) unsigned char device_view_triangle_smem[];
+    constexpr unsigned kFull = 0xFFFFFFFFu;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    bvhb200::SmemStack<U> stack { reinterpret_cast<U*>(device_view_triangle_smem) + threadIdx.x, bvhb200::kTraceBlock, 0 };
+
+    bvhb200::RunCursor run;
+    bool has_ray = false;
+    unsigned long long index = 0;
+    bvhb200::RayCtx<T> r;
+    bvhb200::HitState<T> hit;           // (hit.t is the ray's input tmax until a hit is recorded: a miss's record t)
+    Payload payload;
+    U top = 0;
+    auto retire = [&] {
+        ts.shader.finish(static_cast<size_t>(index), static_cast<const Payload&>(payload),
+                         detail::make_hit<T>(bvhb200::make_record(hit, hit.t, ts.prim_ids)));
+        has_ray = false;
+    };
+
+    // one draw: the idle lanes take the next rays of the warp's run; a ray whose interval is a NaN retires at once as a
+    // miss.  The root's index is read per ray (one L1 hit) rather than held for the whole kernel: that register is what
+    // lets the float kernel fit its 56 without spills.
+    auto draw = [&] (unsigned idle, unsigned rank) {
+        return detail::draw_run(run, cursor, n, run_rays, lane, has_ray, idle, rank, [&] (unsigned long long i) {
+            index = i;
+            detail::load_ray<T>(ts.shader.start(static_cast<size_t>(index), payload), r);
+            hit.slot = bvhb200::kInvalidId; hit.t = r.tmax; hit.u = T(0); hit.v = T(0);
+            if (bvhb200::ray_interval_is_nan(r)) { retire(); return; }
+            bvhb200::ray_prologue<T, IsRobust>(r);
+            top = nodes[1].index;
+            stack.clear();
+            has_ray = true;
+        });
+    };
+
+    // inner phase: descend until this lane holds a leaf, its ray is finished, or the step budget of this round is spent
+    auto inner = [&] {
+        if (has_ray) {
+            uint32_t budget = inner_budget;
+            while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone ends it too)
+                --budget;
+                bvhb200::inner_step<T, IsAnyHit, IsRobust>(nodes, r, top, stack);
+            }
+            if (top == bvhb200::kTraversalDone<U>) retire();
+        }
+    };
+
+    // leaf phase: the leaf's triangles through the shader's filter; the ray ends on an any-hit hit or an empty stack
+    auto leaf = [&] {
+        if (has_ray && bvhb200::index_count(top) != 0) {
+            detail::shader_leaf<T, TieLastVisited>(ts, payload, (uint32_t)bvhb200::index_first(top), bvhb200::index_count(top), r, hit);
+            if ((IsAnyHit && hit.slot != bvhb200::kInvalidId) || !stack.try_pop(top)) retire();
+        }
+    };
+    bvhb200::run_rounds<false>(run, has_ray, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
+                               [] {});
+}
 #endif
 
 // A plain-data view of one device tree (what bvhNN_get_device_view reports), passed to kernels by value.
@@ -514,6 +646,7 @@ template <typename T> struct DeviceView {
     using Scalar = T;
     using Index = typename bvhb200::Real<T>::UInt;      // a node's packed index: first id << 4 | primitive count
     using Ray = typename detail::ViewTypes<T>::Ray;     // bvh_ray3f / bvh_ray3d
+    using Hit = typename detail::ViewTypes<T>::Hit;     // bvh_hit3f / bvh_hit3d: { prim_id; t, u, v }
     using Node = bvhb200::DevNode<T>;                   // { T bounds[6] (minx, maxx, miny, maxy, minz, maxz); Index index; pad }
     using Tri = bvhb200::DevTri<T>;                     // PrecomputedTri: p0, e1 = p0 - p1, e2 = p2 - p0, n = cross(e1, e2)
     template <unsigned Capacity> using SmallStack = bvhb200::ArrayStack<Index, Capacity>;
@@ -648,12 +781,7 @@ template <typename T> struct DeviceView {
     // `on_stream` is a cudaStream_t (unused by the host pass)
     template <bool IsAnyHit, bool IsRobust, typename Tracer>
     void trace(size_t n, const Tracer& tracer, void* workspace, size_t workspace_bytes, void* on_stream) const {
-        // the library's scheduling of a persistent closest-hit or any-hit batch, with its default settings
-        bvhb200::TraceRequest request {};
-        request.flags = bvhb200::kTraceNoTma | (IsAnyHit ? bvhb200::kTraceAnyHit : 0u) | (IsRobust ? bvhb200::kTraceRobust : 0u);
-        request.is_float = sizeof(T) == 4;
-        request.n = n;
-        const bvhb200::TracePlan plan = bvhb200::plan_trace(request);
+        const bvhb200::TracePlan plan = batch_plan<IsAnyHit, IsRobust>(n, 0u);
 #if defined(__CUDACC__)
         run_batch("trace", device_view_trace_kernel<T, IsAnyHit, IsRobust, Tracer>, tracer, n, plan.refill_min, plan.inner_budget,
                   workspace, workspace_bytes, on_stream);
@@ -713,6 +841,50 @@ template <typename T> struct DeviceView {
 #endif
     }
 
+    // A whole batch of rays through the library's triangle traversal, with the caller's ray source, hit filter and hit
+    // sink: see "Whole batches of triangle rays" at the top of this file.  The workspace is the warps' run cursor,
+    // trace_workspace_bytes() bytes.
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_triangles(size_t n, const Shader& shader, void* workspace, size_t workspace_bytes) const {
+        trace_triangles<IsAnyHit, IsRobust, TieLastVisited>(n, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_triangles(size_t n, const Shader& shader, void* workspace, size_t workspace_bytes, void* on_stream) const {
+        if (!tris)
+            throw std::invalid_argument("bvh::v2::cuda::DeviceView::trace_triangles: the tree has no triangles (built from boxes)");
+        const bvhb200::TracePlan plan = batch_plan<IsAnyHit, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
+        const detail::TriangleShader<T, Shader> ts { shader, tris, prim_ids };
+#if defined(__CUDACC__)
+        run_batch("trace_triangles", device_view_triangle_kernel<T, IsAnyHit, IsRobust, TieLastVisited, Shader>, ts, n, plan.refill_min,
+                  plan.inner_budget, workspace, workspace_bytes, on_stream);
+#else
+        (void)on_stream; (void)plan;
+        batch_stack_bytes("trace_triangles", workspace, workspace_bytes);
+        using Payload = typename Shader::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            bvhb200::RayCtx<T> r;
+            load(shader.start(i, payload), r);
+            const T tmax_in = r.tmax;
+            bvhb200::HitState<T> hit { bvhb200::kInvalidId, r.tmax, T(0), T(0) };
+            if (!bvhb200::ray_interval_is_nan(r)) {
+                bvhb200::ray_prologue<T, IsRobust>(r);
+                detail::VectorStack<Index> stack;
+                stack.elems.reserve(stack_bound());
+                bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
+                    nodes, r, root_index(), stack,
+                    [&](Index begin, Index end) {
+                        detail::shader_leaf<T, TieLastVisited>(ts, payload, (uint32_t)begin, (uint32_t)(end - begin), r, hit);
+                        return hit.slot != bvhb200::kInvalidId;
+                    },
+                    [](Index) {});
+            }
+            shader.finish(i, static_cast<const Payload&>(payload), detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, prim_ids)));
+        }
+#endif
+    }
+
     // PrecomputedTri::intersect (reference tri.h:55-74) on BVH-order triangle k: true, with the hit's distance and
     // barycentrics, when the ray meets it at a distance in [ray.tmin, ray.tmax].  The batched kernels' own test.
     BVH_HD bool intersect_tri(size_t k, const Ray& ray, T& t, T& u, T& v) const {
@@ -730,7 +902,17 @@ private:
     // the shared memory a persistent block may have, as bvhNN_intersect_rays bounds it
     static constexpr size_t kMaxTraceSmem = 200 * 1024;
 
-    // The checks of trace and query (`call`): the workspace, then the shared-memory stack of the batched kernels, sized
+    // The library's scheduling of a persistent closest-hit or any-hit batch (trace, trace_triangles), with its default
+    // settings; `flags` adds kTraceLastVisited.
+    template <bool IsAnyHit, bool IsRobust> static bvhb200::TracePlan batch_plan(size_t n, unsigned flags) {
+        bvhb200::TraceRequest request {};
+        request.flags = bvhb200::kTraceNoTma | (IsAnyHit ? bvhb200::kTraceAnyHit : 0u) | (IsRobust ? bvhb200::kTraceRobust : 0u) | flags;
+        request.is_float = sizeof(T) == 4;
+        request.n = n;
+        return bvhb200::plan_trace(request);
+    }
+
+    // The checks of trace, query and trace_triangles (`call`): the workspace, then the shared-memory stack of the batched kernels, sized
     // and bounded as bvhNN_intersect_rays sizes and bounds it.  Returns the stack's bytes per block.
     size_t batch_stack_bytes(const char* call, void* workspace, size_t workspace_bytes) const {
         const std::string who = std::string("bvh::v2::cuda::DeviceView::") + call;
@@ -746,8 +928,9 @@ private:
         return smem;
     }
 #if defined(__CUDACC__)
-    // The launch of trace and query: the checks, then, unless n == 0, the current device switched to the tree's, the run
-    // cursor reset, and one resident wave of `kernel` (device_view_trace_kernel or device_view_query_kernel) on
+    // The launch of trace, query and trace_triangles: the checks, then, unless n == 0, the current device switched to the
+    // tree's, the run cursor reset, and one resident wave of `kernel` (device_view_trace_kernel, device_view_query_kernel or
+    // device_view_triangle_kernel) on
     // `on_stream` with the run length and grid of bvhNN_intersect_rays' persistent kernel.
     template <typename Fn>
     void run_batch(const char* call, void (*kernel)(const Node*, unsigned long long, unsigned long long*, uint32_t, uint32_t, uint32_t, Fn),
