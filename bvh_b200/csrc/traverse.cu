@@ -794,17 +794,23 @@ int make_ray_order(const DeviceBvh<T>& bvh, const DevRay<T>* d_rays, uint32_t n,
     return 0;
 }
 
+// The most dynamic shared memory a trace launch may ask for (stack, TMA and staging areas together).
+constexpr size_t kMaxTraceSmem = 200 * 1024;
+
+// The kernel's dynamic shared-memory limit is a process-wide attribute of the function, not of the call: it is always
+// raised to kMaxTraceSmem, never to this call's size, so that a concurrent call on a shallower tree cannot lower it
+// between another thread's setting and launch.
 template <typename KernelT>
 int configure_smem(KernelT kernel, size_t smem_bytes) {
     if (smem_bytes > 48 * 1024)
-        BVH_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+        BVH_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxTraceSmem));
     return 0;
 }
 
 // One resident wave of persistent CTAs (SM count x occupancy), never more than the batch can feed.
 template <typename KernelT, typename T>
 int launch_persistent(KernelT kernel, const TraceArgs<T>& args, size_t smem, unsigned rays_per_warp, int device, cudaStream_t stream) {
-    if (smem > 200 * 1024) { set_error("trace: tree too deep for the shared-memory stack"); return -1; }
+    if (smem > kMaxTraceSmem) { set_error("trace: tree too deep for the shared-memory stack"); return -1; }
     if (configure_smem(kernel, smem)) return -1;
     if (const int carve = tunables().smem_carveout.load(); carve >= 0)
         BVH_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve));
@@ -823,7 +829,7 @@ template <typename T, bool kAny, bool kRobust>
 int launch(TraceKernel kernel, const TraceArgs<T>& args, bool staged, int device, cudaStream_t stream) {
     using U = typename Real<T>::UInt;
     size_t smem = (size_t)args.stack_entries * kTraceBlock * sizeof(U);
-    if (smem > 200 * 1024) { set_error("trace: tree too deep for the shared-memory stack"); return -1; }
+    if (smem > kMaxTraceSmem) { set_error("trace: tree too deep for the shared-memory stack"); return -1; }
     const size_t stage = staged ? stage_smem_bytes<T>() : 0;
     void (*persistent)(TraceArgs<T>) = nullptr;
     unsigned rays_per_warp = 32;

@@ -944,7 +944,10 @@ private:
         if (previous != device) check(cudaSetDevice(device), "cudaSetDevice", call);
         int sm_count = 0, per_sm = 0;
         cudaError_t e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device);
-        if (e == cudaSuccess && smem > 48 * 1024) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        // (the limit belongs to the kernel function, shared by every caller in the process: always kMaxTraceSmem, so that a
+        // concurrent batch on a shallower tree cannot lower it under this launch)
+        if (e == cudaSuccess && smem > 48 * 1024)
+            e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxTraceSmem);
         if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, bvhb200::kTraceBlock, smem);
         if (e == cudaSuccess) e = cudaMemsetAsync(workspace, 0, trace_workspace_bytes(), s);
         if (e == cudaSuccess) {
