@@ -74,6 +74,8 @@ QUERY_BATCH_KERNELS_SRC = os.path.join(ROOT, "tests", "device_query_batch_kernel
 QUERY_BATCH_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_query_batch_kernels.so")
 TRIANGLE_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_triangle_trace_kernels.cu")
 TRIANGLE_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_triangle_trace_kernels.so")
+PATH_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_path_trace_kernels.cu")
+PATH_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_path_trace_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -134,6 +136,13 @@ def build_device_triangle_trace_tests(force: bool = False, verbose: bool = False
     """tests/device_triangle_trace_kernels.cu: the test shaders of DeviceView::trace_triangles (recording filters, the
     plain array shader, an in-kernel camera) and the same filters one thread per ray."""
     return _build_test_kernels(TRIANGLE_TRACE_KERNELS_SRC, TRIANGLE_TRACE_KERNELS_LIB, force, verbose)
+
+
+def build_device_path_trace_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_path_trace_kernels.cu: the test shaders of DeviceView::trace_paths (a path tracer with next-event
+    shadow segments, as one call and as a wavefront loop of trace_triangles; a recording shader of scripted segments)
+    and the same segments one thread each."""
+    return _build_test_kernels(PATH_TRACE_KERNELS_SRC, PATH_TRACE_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

@@ -309,6 +309,65 @@
 //     };
 //     view.trace_triangles<true, false>(n, ShadowShader { d_rays, d_origins, d_lit }, workspace, bytes, stream);
 //
+// Whole paths: view.trace_paths<IsRobust, TieLastVisited = false>(n, shader, workspace, workspace_bytes[, stream]) traces
+// paths 0 .. n-1, each a sequence of triangle-ray segments (bounce and shadow rays of a path tracer, ambient occlusion
+// with bounces, acoustics), in one launch: when a segment ends, its lane starts the path's next segment in place, with
+// the same payload registers and the same shared-memory stack; only lanes whose path is over are refilled.  What OptiX
+// calls tracing from closest-hit, reduced to the library's semantics.  The shader is a plain struct copied to the kernel
+// by value, with a Payload type (per-path state, kept in registers) and four __device__ (or __host__ __device__)
+// functions:
+//     PathStep start(size_t i, Payload& p, Ray& ray) const;                     // first segment of path i, or End
+//     bool     accept(Payload& p, size_t prim_id, T t, T u, T v) const;         // exactly as in trace_triangles
+//     PathStep next(size_t i, Payload& p, const Hit& hit, Ray& ray) const;      // a segment ended: the next one, or End
+//     void     finish(size_t i, const Payload& p) const;                        // path i is done
+// PathStep is End, Closest or Occlusion.
+//   * for every i in [0, n), start is called once, then zero or more segments, then finish once.  If start returns End,
+//     finish follows directly;
+//   * each segment is what trace_triangles does for that ray: a Closest segment is trace_triangles<false, IsRobust,
+//     TieLastVisited>, an Occlusion segment trace_triangles<true, IsRobust, TieLastVisited>.  It gets the same accept
+//     calls, with the same ids and the same bits of t, u and v, in the same order, and then next with the record
+//     trace_triangles would hand to finish.  A segment whose interval is a NaN gets no accept call and a miss record;
+//   * on entry to next, `ray` is the segment's ray as start or the previous next returned it, not shrunk by the
+//     traversal.  On a return other than End, `ray` is the next segment;
+//   * the payload lives across segments.  Different paths may be in different segment kinds in the same warp;
+//   * the other rules are those of trace_triangles: no __syncthreads and no full-mask collectives in shader code; no
+//     watchdog (a shader that never returns End never ends); stream-ordered, setting and restoring the current device;
+//     n == 0 launches nothing; workspace: view.trace_workspace_bytes() bytes.  A smaller workspace or a tree too deep for
+//     the 200 KB shared-memory stack throws std::length_error, a view without triangles std::invalid_argument, a failed
+//     launch std::runtime_error;
+//   * scheduling uses plan_trace's closest-hit settings for the whole batch, with grid and run length from n;
+//   * compiled as plain host C++, the paths run serially, each segment through the host code of one trace_triangles ray.
+// The kernel is bvh::v2::cuda::device_view_path_kernel<T, IsRobust, TieLastVisited, Shader>, with trace_triangles'
+// launch bounds, block, stack and phases; a lane's segment kind picks the any-hit or closest-hit inner step.  The payload
+// competes with the traversal for the float kernel's 56 registers: keep it to a few words.  A grey diffuse path tracer
+// with a point light and next-event estimation (INTEGRATION.md §5 has it whole):
+//
+//     struct PathTracer {
+//         struct Payload { float throughput, radiance, pending; uint32_t prim, bounce; };   // pending: the shadow ray's share
+//         ...                                                                 // camera, light, normals, radiance out
+//         __device__ PathStep start(size_t i, Payload& p, bvh_ray3f& ray) const {
+//             ray = camera_ray(i); p = { 1.0f, 0.0f, 0.0f, UINT32_MAX, 0 };
+//             return PathStep::Closest;
+//         }
+//         __device__ bool accept(Payload& p, size_t prim_id, float, float, float) const { return prim_id != p.prim; }
+//         __device__ PathStep next(size_t i, Payload& p, const bvh_hit3f& hit, bvh_ray3f& ray) const {
+//             if (p.pending != 0.0f) {                                       // a shadow segment ended
+//                 if (hit.prim_id == UINT32_MAX) p.radiance += p.pending;
+//                 p.pending = 0.0f;
+//                 return bounce(i, p, ray);                                  // ray.org is the surface point
+//             }
+//             if (hit.prim_id == UINT32_MAX) { p.radiance += p.throughput * sky; return PathStep::End; }
+//             p.prim = hit.prim_id;
+//             ray.org = ray.org + hit.t * ray.dir;                           // the surface point
+//             p.pending = light_share(p, ray.org);                           // 0 when the light is behind the surface
+//             if (p.pending == 0.0f) return bounce(i, p, ray);
+//             ray.dir = light - ray.org; ray.tmin = 0.0f; ray.tmax = 1.0f;
+//             return PathStep::Occlusion;
+//         }
+//         __device__ void finish(size_t i, const Payload& p) const { image[i] = p.radiance; }
+//     };
+//     view.trace_paths<false>(width * height, PathTracer { ... }, workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -333,6 +392,10 @@
 #include "traverse_core.cuh"
 
 namespace bvh::v2::cuda {
+
+// What a path shader of DeviceView::trace_paths asks for next: the path's end, a closest-hit segment or an occlusion
+// (any-hit) segment.
+enum class PathStep { End, Closest, Occlusion };
 
 namespace detail {
 template <typename T> struct ViewTypes;
@@ -639,6 +702,102 @@ device_view_triangle_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsig
     bvhb200::run_rounds<false>(run, has_ray, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
                                [] {});
 }
+
+// The kernel of DeviceView::trace_paths: device_view_triangle_kernel's scheduler, launch settings, stack and phases, with
+// a path per lane instead of a ray.  A lane draws path i through shader.start; each segment runs the any-hit or the
+// closest-hit inner step by the lane's segment kind; when a segment ends (leaf phase) the lane hands its record to
+// shader.next and either re-arms in place for the next segment, keeping its payload, or retires the path through
+// shader.finish.  Only lanes whose path is over become idle and are refilled.
+template <typename T, bool IsRobust, bool TieLastVisited, typename Shader>
+__global__ void __launch_bounds__(bvhb200::kTraceBlock, sizeof(T) == 4 ? BVH_TRACE_BLOCKS : 4)
+device_view_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned long long n, unsigned long long* cursor,
+                        uint32_t run_rays, uint32_t refill_min, uint32_t inner_budget, detail::TriangleShader<T, Shader> ts) {
+    using U = typename bvhb200::Real<T>::UInt;
+    using Payload = typename Shader::Payload;
+    using Ray = typename detail::ViewTypes<T>::Ray;
+    extern __shared__ __align__(128) unsigned char device_view_path_smem[];
+    constexpr unsigned kFull = 0xFFFFFFFFu;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    bvhb200::SmemStack<U> stack { reinterpret_cast<U*>(device_view_path_smem) + threadIdx.x, bvhb200::kTraceBlock, 0 };
+
+    bvhb200::RunCursor run;
+    bool has_path = false;
+    unsigned long long index = 0;
+    bvhb200::RayCtx<T> r;
+    bvhb200::HitState<T> hit;
+    T tmax_in = T(0);                   // the segment's tmax as the shader gave it (r.tmax shrinks on hits)
+    bool occlusion = false;             // the segment's kind: any-hit inner step, ends on its first accepted hit
+    Payload payload;
+    U top = 0;
+    auto retire = [&] {
+        ts.shader.finish(static_cast<size_t>(index), static_cast<const Payload&>(payload));
+        has_path = false;
+    };
+
+    // the lane's next segment: hit state reset, prologue, root, empty stack.  A segment whose interval is a NaN gets no
+    // traversal: it starts at kTraversalDone and ends as a miss in the next leaf phase, with no accept call.
+    auto arm = [&](PathStep step, const Ray& ray) {
+        detail::load_ray<T>(ray, r);
+        tmax_in = r.tmax;
+        hit.slot = bvhb200::kInvalidId; hit.t = r.tmax; hit.u = T(0); hit.v = T(0);
+        occlusion = step == PathStep::Occlusion;
+        top = bvhb200::kTraversalDone<U>;
+        if (!bvhb200::ray_interval_is_nan(r)) {
+            bvhb200::ray_prologue<T, IsRobust>(r);
+            top = nodes[1].index;       // (read per segment, as device_view_triangle_kernel reads it per ray)
+        }
+        stack.clear();
+        has_path = true;
+    };
+
+    // a segment ended: its record and its ray as the shader gave it to next, then the next segment or the path's end
+    auto end_segment = [&] {
+        Ray ray = detail::make_ray<Ray>(r);
+        ray.tmax = tmax_in;
+        const PathStep step = ts.shader.next(static_cast<size_t>(index), payload,
+                                             detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, ts.prim_ids)), ray);
+        if (step == PathStep::End) retire();
+        else arm(step, ray);
+    };
+
+    // one draw: the idle lanes take the next paths of the warp's run
+    auto draw = [&] (unsigned idle, unsigned rank) {
+        return detail::draw_run(run, cursor, n, run_rays, lane, has_path, idle, rank, [&] (unsigned long long i) {
+            index = i;
+            Ray ray;
+            const PathStep step = ts.shader.start(static_cast<size_t>(index), payload, ray);
+            if (step == PathStep::End) retire();
+            else arm(step, ray);
+        });
+    };
+
+    // inner phase: descend until this lane holds a leaf, its segment is finished, or the step budget of this round is spent
+    auto inner = [&] {
+        if (has_path) {
+            uint32_t budget = inner_budget;
+            while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone ends it too)
+                --budget;
+                if (occlusion) bvhb200::inner_step<T, true, IsRobust>(nodes, r, top, stack);
+                else bvhb200::inner_step<T, false, IsRobust>(nodes, r, top, stack);
+            }
+        }
+    };
+
+    // leaf phase: the leaf's triangles through the shader's filter; the segment ends on an occlusion hit, an empty stack,
+    // or when the inner phase found nothing left (kTraversalDone)
+    auto leaf = [&] {
+        if (!has_path) return;
+        bool ended = top == bvhb200::kTraversalDone<U>;
+        if (!ended && bvhb200::index_count(top) != 0) {
+            detail::shader_leaf<T, TieLastVisited>(ts, payload, (uint32_t)bvhb200::index_first(top), bvhb200::index_count(top), r, hit);
+            ended = (occlusion && hit.slot != bvhb200::kInvalidId) || !stack.try_pop(top);
+        }
+        if (ended) end_segment();
+    };
+    bvhb200::run_rounds<false>(run, has_path, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
+                               [] {});
+}
 #endif
 
 // A plain-data view of one device tree (what bvhNN_get_device_view reports), passed to kernels by value.
@@ -864,23 +1023,42 @@ template <typename T> struct DeviceView {
         using Payload = typename Shader::Payload;
         for (size_t i = 0; i < n; ++i) {
             Payload payload;
-            bvhb200::RayCtx<T> r;
-            load(shader.start(i, payload), r);
-            const T tmax_in = r.tmax;
-            bvhb200::HitState<T> hit { bvhb200::kInvalidId, r.tmax, T(0), T(0) };
-            if (!bvhb200::ray_interval_is_nan(r)) {
-                bvhb200::ray_prologue<T, IsRobust>(r);
-                detail::VectorStack<Index> stack;
-                stack.elems.reserve(stack_bound());
-                bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
-                    nodes, r, root_index(), stack,
-                    [&](Index begin, Index end) {
-                        detail::shader_leaf<T, TieLastVisited>(ts, payload, (uint32_t)begin, (uint32_t)(end - begin), r, hit);
-                        return hit.slot != bvhb200::kInvalidId;
-                    },
-                    [](Index) {});
+            const Ray ray = shader.start(i, payload);
+            shader.finish(i, static_cast<const Payload&>(payload), host_triangle_ray<IsAnyHit, IsRobust, TieLastVisited>(ts, payload, ray));
+        }
+#endif
+    }
+
+    // Whole paths of triangle-ray segments, each continued in place from the last: see "Whole paths" at the top of this
+    // file.  The workspace is the warps' run cursor, trace_workspace_bytes() bytes.
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_paths(size_t n, const Shader& shader, void* workspace, size_t workspace_bytes) const {
+        trace_paths<IsRobust, TieLastVisited>(n, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_paths(size_t n, const Shader& shader, void* workspace, size_t workspace_bytes, void* on_stream) const {
+        if (!tris)
+            throw std::invalid_argument("bvh::v2::cuda::DeviceView::trace_paths: the tree has no triangles (built from boxes)");
+        const bvhb200::TracePlan plan = batch_plan<false, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
+        const detail::TriangleShader<T, Shader> ts { shader, tris, prim_ids };
+#if defined(__CUDACC__)
+        run_batch("trace_paths", device_view_path_kernel<T, IsRobust, TieLastVisited, Shader>, ts, n, plan.refill_min,
+                  plan.inner_budget, workspace, workspace_bytes, on_stream);
+#else
+        (void)on_stream; (void)plan;
+        batch_stack_bytes("trace_paths", workspace, workspace_bytes);
+        using Payload = typename Shader::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            Ray ray;
+            PathStep step = shader.start(i, payload, ray);
+            while (step != PathStep::End) {
+                const Hit hit = step == PathStep::Occlusion ? host_triangle_ray<true, IsRobust, TieLastVisited>(ts, payload, ray)
+                                                            : host_triangle_ray<false, IsRobust, TieLastVisited>(ts, payload, ray);
+                step = shader.next(i, payload, hit, ray);
             }
-            shader.finish(i, static_cast<const Payload&>(payload), detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, prim_ids)));
+            shader.finish(i, static_cast<const Payload&>(payload));
         }
 #endif
     }
@@ -902,7 +1080,7 @@ private:
     // the shared memory a persistent block may have, as bvhNN_intersect_rays bounds it
     static constexpr size_t kMaxTraceSmem = 200 * 1024;
 
-    // The library's scheduling of a persistent closest-hit or any-hit batch (trace, trace_triangles), with its default
+    // The library's scheduling of a persistent closest-hit or any-hit batch (trace, trace_triangles, trace_paths), with its default
     // settings; `flags` adds kTraceLastVisited.
     template <bool IsAnyHit, bool IsRobust> static bvhb200::TracePlan batch_plan(size_t n, unsigned flags) {
         bvhb200::TraceRequest request {};
@@ -912,7 +1090,31 @@ private:
         return bvhb200::plan_trace(request);
     }
 
-    // The checks of trace, query and trace_triangles (`call`): the workspace, then the shared-memory stack of the batched kernels, sized
+    // One ray of trace_triangles, and one segment of trace_paths, on the host: the library's traversal with the shader's
+    // accept as the leaf's filter, and the record finish (trace_triangles) or next (trace_paths) receives.  A ray whose
+    // interval is a NaN gets no accept call and a miss record.
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited, typename Shader, typename Payload>
+    Hit host_triangle_ray(const detail::TriangleShader<T, Shader>& ts, Payload& payload, const Ray& ray) const {
+        bvhb200::RayCtx<T> r;
+        load(ray, r);
+        const T tmax_in = r.tmax;
+        bvhb200::HitState<T> hit { bvhb200::kInvalidId, r.tmax, T(0), T(0) };
+        if (!bvhb200::ray_interval_is_nan(r)) {
+            bvhb200::ray_prologue<T, IsRobust>(r);
+            detail::VectorStack<Index> stack;
+            stack.elems.reserve(stack_bound());
+            bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
+                nodes, r, root_index(), stack,
+                [&](Index begin, Index end) {
+                    detail::shader_leaf<T, TieLastVisited>(ts, payload, (uint32_t)begin, (uint32_t)(end - begin), r, hit);
+                    return hit.slot != bvhb200::kInvalidId;
+                },
+                [](Index) {});
+        }
+        return detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, prim_ids));
+    }
+
+    // The checks of trace, query, trace_triangles and trace_paths (`call`): the workspace, then the shared-memory stack of the batched kernels, sized
     // and bounded as bvhNN_intersect_rays sizes and bounds it.  Returns the stack's bytes per block.
     size_t batch_stack_bytes(const char* call, void* workspace, size_t workspace_bytes) const {
         const std::string who = std::string("bvh::v2::cuda::DeviceView::") + call;
@@ -928,10 +1130,10 @@ private:
         return smem;
     }
 #if defined(__CUDACC__)
-    // The launch of trace, query and trace_triangles: the checks, then, unless n == 0, the current device switched to the
-    // tree's, the run cursor reset, and one resident wave of `kernel` (device_view_trace_kernel, device_view_query_kernel or
-    // device_view_triangle_kernel) on
-    // `on_stream` with the run length and grid of bvhNN_intersect_rays' persistent kernel.
+    // The launch of trace, query, trace_triangles and trace_paths: the checks, then, unless n == 0, the current device
+    // switched to the tree's, the run cursor reset, and one resident wave of `kernel` (device_view_trace_kernel,
+    // device_view_query_kernel, device_view_triangle_kernel or device_view_path_kernel) on `on_stream` with the run length
+    // and grid of bvhNN_intersect_rays' persistent kernel.
     template <typename Fn>
     void run_batch(const char* call, void (*kernel)(const Node*, unsigned long long, unsigned long long*, uint32_t, uint32_t, uint32_t, Fn),
                    const Fn& fn, size_t n, uint32_t refill_min, uint32_t inner_budget, void* workspace, size_t workspace_bytes,
