@@ -76,6 +76,8 @@ TRIANGLE_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_triangle_trace_
 TRIANGLE_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_triangle_trace_kernels.so")
 PATH_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_path_trace_kernels.cu")
 PATH_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_path_trace_kernels.so")
+INSTANCE_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_instance_trace_kernels.cu")
+INSTANCE_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_instance_trace_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -143,6 +145,13 @@ def build_device_path_trace_tests(force: bool = False, verbose: bool = False) ->
     shadow segments, as one call and as a wavefront loop of trace_triangles; a recording shader of scripted segments)
     and the same segments one thread each."""
     return _build_test_kernels(PATH_TRACE_KERNELS_SRC, PATH_TRACE_KERNELS_LIB, force, verbose)
+
+
+def build_device_instance_trace_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_instance_trace_kernels.cu: the test shaders of DeviceView::trace_instances and prepare_instances (a
+    recording shader, the same rays nested by hand one thread each, the benchmark's plain shaders and a hand-nested
+    DeviceView::trace tracer)."""
+    return _build_test_kernels(INSTANCE_TRACE_KERNELS_SRC, INSTANCE_TRACE_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

@@ -368,6 +368,61 @@
 //     };
 //     view.trace_paths<false>(width * height, PathTracer { ... }, workspace, bytes, stream);
 //
+// Instanced scenes: top.trace_instances<IsAnyHit, IsRobust, TieLastVisited = false>(n, instances, shader, workspace,
+// workspace_bytes[, stream]) traces triangle rays through a two-level scene: each distinct mesh keeps its own tree (built
+// once with bvhNN_build_triangles), and `top` is a tree over the world boxes of its placed copies.  An Instance<T> record
+// (make_instance(view, object_to_world)) holds a bottom tree's device arrays, its root and depth, a 3 x 4 row-major
+// object_to_world matrix the caller writes and its inverse world_to_object; Instances<T> { records, count, max_depth }
+// views count records in device memory, max_depth being the largest bottom depth.  prepare_instances(instances, bboxes,
+// centers[, stream]) writes every root index and world_to_object, and the world boxes and centres (bvh_bbox3f / bvh_vec3f, or 3d) that
+// bvhNN_build_boxes or bvhNN_refit_boxes take with BVH_DEVICE_POINTERS, in one stream-ordered kernel.  Top primitive k is
+// record k: build the top tree from those arrays, then for a rigid move rewrite object_to_world, prepare_instances and
+// refit_boxes on the top handle's stream, and trace.  The shader is a plain struct copied to the kernel by value, with a
+// Payload type and three __device__ (or __host__ __device__) functions:
+//     Ray  start(size_t i, Payload& p) const;                                          // ray i of the batch (world space)
+//     bool accept(Payload& p, uint32_t instance, size_t prim_id, T t, T u, T v) const;  // a candidate hit; false: ignore it
+//     void finish(size_t i, const Payload& p, const Hit& hit, uint32_t instance) const; // ray i is done; all ones: a miss
+//   * for every i in [0, n), start once, then the accept calls, then finish once.  They are exactly the calls of this host
+//     loop, which is what the header compiled as plain host C++ runs: Bvh::intersect<IsAnyHit, IsRobust> on the top tree,
+//     whose leaf takes the leaf's instances in BVH order and, for each, transforms the world ray by world_to_object
+//     (origin as a point, direction as a vector, tmin and tmax unchanged: detail::object_ray), runs the instance's
+//     Bvh::intersect<IsAnyHit, IsRobust> with a PrecomputedTri::intersect leaf, the tie rule and accept as the filter, and
+//     carries the shrunk tmax back to the top level.  An instance whose world_to_object is NaN (no inverse) is skipped;
+//   * t is the world ray's parameter (the object ray is not normalised); u and v are the object-space barycentrics;
+//     prim_id is the bottom mesh's original id; `instance` is the record's index;
+//   * tie rule: at an exact tie in t the canonical rule keeps the lower instance, then the lower original id; with
+//     TieLastVisited the last visited candidate wins.  true from accept records the hit and shrinks tmax; with IsAnyHit
+//     the ray ends after the bottom leaf that accepted it.  A ray whose interval is a NaN finishes at once as a miss with
+//     no accept call.  finish receives the record of trace_triangles (id, t, u, v; on a miss all ones, the input tmax, 0,
+//     0) and the hit's instance;
+//   * with one instance whose matrix is the identity (its world box a top tree of one leaf), the accept calls and the
+//     record are those of trace_triangles on that mesh, bit for bit: detail::affine_row maps coordinates exactly through
+//     an identity, a permutation or a power-of-two scale;
+//   * errors, checked on the host before any launch: instances.count other than the top tree's prim_count throws
+//     std::invalid_argument; a stack of top depth + max_depth + 9 entries per ray beyond the 200 KB shared-memory stack,
+//     or a small workspace, std::length_error; a failed launch std::runtime_error.  That every record's bottom view has
+//     triangles, outlives the call and that max_depth is right is the caller's, like the view-lifetime rules;
+//   * streams, the workspace (trace_workspace_bytes()), n == 0, the warp subset and the watchdog are those of
+//     trace_triangles.  Compiled as plain host C++, the rays run serially through the nested loop above.
+// The kernel is bvh::v2::cuda::device_view_instance_kernel<T, IsAnyHit, IsRobust, TieLastVisited, Shader>, with
+// trace_triangles' launch bounds, block, scheduling and launch: each lane walks both levels in one stack machine on its
+// shared-memory stack (DESIGN.md §8 has the layout).  Two meshes, three copies, one frame (INTEGRATION.md §5 has it whole):
+//
+//     struct Shade {
+//         struct Payload {};
+//         const bvh_ray3f* rays; bvh_hit3f* hits; uint32_t* inst;
+//         __device__ bvh_ray3f start(size_t i, Payload&) const { return rays[i]; }
+//         __device__ bool accept(Payload&, uint32_t, size_t, float, float, float) const { return true; }
+//         __device__ void finish(size_t i, const Payload&, const bvh_hit3f& h, uint32_t k) const { hits[i] = h; inst[i] = k; }
+//     };
+//     Instance<float> recs[3] = { make_instance(rock, m0), make_instance(rock, m1), make_instance(tree, m2) };  // host
+//     cudaMemcpyAsync(d_recs, recs, sizeof recs, cudaMemcpyHostToDevice, stream);
+//     const Instances<float> instances { d_recs, 3, std::max(rock.depth, tree.depth) };
+//     prepare_instances(instances, d_boxes, d_centres, stream);
+//     bvh3f* top_bvh = bvh3f_build_boxes(d_boxes, d_centres, 3, nullptr, BVH_DEVICE_POINTERS);   // once; later frames:
+//     // bvh3f_refit_boxes(top_bvh, d_boxes, 3, BVH_DEVICE_POINTERS) after prepare_instances on the top handle's stream
+//     top.trace_instances<false, false>(n, instances, Shade { d_rays, d_hits, d_inst }, workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -397,10 +452,36 @@ namespace bvh::v2::cuda {
 // (any-hit) segment.
 enum class PathStep { End, Closest, Occlusion };
 
+// One placed copy of a triangle mesh for DeviceView::trace_instances: the bottom tree's device arrays (from a DeviceView
+// with triangles), its root and depth, and the placement.  Fill it with make_instance(view, object_to_world) and keep the
+// records in device memory of the caller's.  object_to_world is the caller's; root_index and world_to_object are written
+// by prepare_instances (all NaN for a matrix that has no inverse, which trace_instances then skips).
+template <typename T> struct alignas(16) Instance {
+    const bvhb200::DevNode<T>* nodes;   // the bottom view's nodes, prim_ids (BVH order) and tris (BVH order)
+    const uint32_t* prim_ids;
+    const bvhb200::DevTri<T>* tris;
+    typename bvhb200::Real<T>::UInt root_index;     // the bottom root's index, written by prepare_instances
+    uint32_t depth;                     // the bottom tree's depth
+    T object_to_world[12];              // 3 x 4 row-major affine: world = A * object + b, row i = A[i][0..2], b[i]
+    T world_to_object[12];              // its inverse, same layout
+};
+
+// A plain view of `count` instance records in device memory.  max_depth is the largest bottom depth among them: the
+// host sizes the shared-memory stack of trace_instances from it.
+template <typename T> struct Instances {
+    Instance<T>* records = nullptr;
+    size_t count = 0;
+    size_t max_depth = 0;
+};
+
 namespace detail {
 template <typename T> struct ViewTypes;
-template <> struct ViewTypes<float>  { using CView = bvh_device_view3f; using Ray = bvh_ray3f; using Hit = bvh_hit3f; };
-template <> struct ViewTypes<double> { using CView = bvh_device_view3d; using Ray = bvh_ray3d; using Hit = bvh_hit3d; };
+template <> struct ViewTypes<float>  {
+    using CView = bvh_device_view3f; using Ray = bvh_ray3f; using Hit = bvh_hit3f; using BBox = bvh_bbox3f; using Vec = bvh_vec3f;
+};
+template <> struct ViewTypes<double> {
+    using CView = bvh_device_view3d; using Ray = bvh_ray3d; using Hit = bvh_hit3d; using BBox = bvh_bbox3d; using Vec = bvh_vec3d;
+};
 struct NoInnerFn { template <typename I> BVH_HD void operator()(I) const {} };
 template <typename T, typename Ray> BVH_HD void load_ray(const Ray& ray, bvhb200::RayCtx<T>& r) {
     r.org[0] = ray.org.x; r.org[1] = ray.org.y; r.org[2] = ray.org.z;
@@ -463,6 +544,125 @@ BVH_HD void shader_leaf(const TriangleShader<T, Shader>& ts, Payload& payload, u
                            [&](uint32_t slot, T t, T u, T v) {
                                return static_cast<bool>(ts.shader.accept(payload, static_cast<size_t>(ts.prim_ids[slot]), t, u, v));
                            });
+}
+
+// What the kernel of DeviceView::trace_instances reads besides the top tree's nodes: the caller's shader, the instance
+// records and the top tree's prim_ids (BVH-order slot -> record).
+template <typename T, typename Shader> struct InstanceShader {
+    Shader shader;
+    const Instance<T>* records;
+    const uint32_t* prim_ids;
+};
+// The instance trace_instances reports for a miss
+constexpr uint32_t kNoInstance = 0xFFFFFFFFu;
+// The stack entry below an instance's bottom traversal: a leaf of 14 primitives at the last representable position,
+// which no tree has (kTraversalDone is the one of 15), so the inner loops stop on it as on a leaf.
+template <typename U> constexpr U kInstanceMarker = bvhb200::kTraversalDone<U> - 1;
+// Stack entries an instance visit adds to the two trees' own: the rest of the top leaf, the world ray's origin and
+// direction (6), the marker, and the bottom traversal's one entry beyond its depth.
+constexpr size_t kInstanceStackExtra = 9;
+
+// Row `row` of a 3 x 4 affine map (row[3] the translation) applied to a point (with the translation) or a vector
+// (without).  The sum starts from -0, the identity of IEEE addition, and skips terms whose coefficient is 0, so a
+// coordinate mapped by an identity, permutation or power-of-two-scale row keeps its exact bits (signed zeros included).
+template <typename T> BVH_HD T affine_row(const T* row, const T p[3], bool point) {
+    using R = bvhb200::Real<T>;
+    T acc = R::neg(T(0));
+    for (int j = 0; j < 3; ++j)
+        if (row[j] != T(0)) acc = R::add(acc, R::mul(row[j], p[j]));
+    if (point && row[3] != T(0)) acc = R::add(acc, row[3]);
+    return acc;
+}
+// The object-space ray of an instance (both builds): the world origin as a point and the direction as a vector through
+// world_to_object, tmin and tmax unchanged, so t keeps its meaning.  `obj` may be `world`.
+template <typename T> BVH_HD void object_ray(const T* world_to_object, const bvhb200::RayCtx<T>& world, bvhb200::RayCtx<T>& obj) {
+    T org[3], dir[3];
+    for (int i = 0; i < 3; ++i) {
+        org[i] = affine_row(world_to_object + 4 * i, world.org, true);
+        dir[i] = affine_row(world_to_object + 4 * i, world.dir, false);
+    }
+    for (int i = 0; i < 3; ++i) { obj.org[i] = org[i]; obj.dir[i] = dir[i]; }
+    obj.tmin = world.tmin; obj.tmax = world.tmax;
+}
+// An instance trace_instances skips: prepare_instances found no inverse (its world_to_object is NaN)
+template <typename T> BVH_HD bool instance_is_singular(const T* world_to_object) { return world_to_object[0] != world_to_object[0]; }
+
+// prepare_instances for one record (both builds).  root_index: the bottom root's.  world_to_object: the adjugate of A over its determinant, then
+// -(A^-1 b); all NaN when an entry of object_to_world is not finite, the determinant is 0 or not finite, or an entry of
+// the inverse is not finite.  The world box of the bottom root box [lo, hi]: per axis i, b_i plus the sums of
+// min / max(a_ij lo_j, a_ij hi_j), which in exact arithmetic is the box of the eight transformed corners.  Its rounding
+// error is below 2.5 eps S_i, S_i = |b_i| + sum_j |a_ij| max(|lo_j|, |hi_j|), so each side is moved out by
+// 4 eps S_i + the smallest normal number (for underflow): the box contains the exact image of the root box.  An empty
+// box (min = +inf, max = -inf) and a zero centre for a matrix without an inverse.
+template <typename T>
+BVH_HD void prepare_instance(Instance<T>& rec, typename ViewTypes<T>::BBox& box, typename ViewTypes<T>::Vec& centre) {
+    using R = bvhb200::Real<T>;
+    using UI = typename R::UInt;
+    const T inf = R::from_bits(sizeof(T) == 4 ? (UI)0x7F800000u : (UI)0x7FF0000000000000ull);
+    const T nan = R::from_bits(~(UI)0 >> 1);
+    const T* m = rec.object_to_world;
+    bool ok = true;
+    for (int k = 0; k < 12; ++k) ok = ok && R::is_finite(m[k]);
+    const T a[3][3] = { { m[0], m[1], m[2] }, { m[4], m[5], m[6] }, { m[8], m[9], m[10] } };
+    T c[3][3];                          // cofactors
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) {
+            const int i1 = (i + 1) % 3, i2 = (i + 2) % 3, j1 = (j + 1) % 3, j2 = (j + 2) % 3;
+            c[i][j] = R::sub(R::mul(a[i1][j1], a[i2][j2]), R::mul(a[i1][j2], a[i2][j1]));
+        }
+    const T det = bvhb200::dot3(a[0], c[0]);
+    ok = ok && det != T(0) && R::is_finite(det);
+    T inv[12];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) inv[4 * i + j] = R::div(c[j][i], det);
+    const T b[3] = { m[3], m[7], m[11] };
+    for (int i = 0; i < 3; ++i) inv[4 * i + 3] = R::neg(affine_row(inv + 4 * i, b, false));
+    for (int k = 0; k < 12; ++k) ok = ok && R::is_finite(inv[k]);
+    for (int k = 0; k < 12; ++k) rec.world_to_object[k] = ok ? inv[k] : nan;
+
+    rec.root_index = rec.nodes[1].index;
+    const T* rb = rec.nodes[1].bounds;  // the bottom root box: minx, maxx, miny, maxy, minz, maxz
+    const T pad = R::mul(R::eps(), T(4)), tiny = sizeof(T) == 4 ? (T)FLT_MIN : (T)DBL_MIN;
+    T lo[3], hi[3], mid[3];
+    for (int i = 0; i < 3; ++i) {
+        T l = m[4 * i + 3], h = m[4 * i + 3], s = R::abs(m[4 * i + 3]);
+        for (int j = 0; j < 3; ++j) {
+            const T p = R::mul(m[4 * i + j], rb[2 * j]), q = R::mul(m[4 * i + j], rb[2 * j + 1]);
+            l = R::add(l, p < q ? p : q);
+            h = R::add(h, p < q ? q : p);
+            const T e = R::abs(rb[2 * j]) < R::abs(rb[2 * j + 1]) ? R::abs(rb[2 * j + 1]) : R::abs(rb[2 * j]);
+            s = R::add(s, R::mul(R::abs(m[4 * i + j]), e));
+        }
+        const T d = R::add(R::mul(s, pad), tiny);
+        lo[i] = R::sub(l, d);
+        hi[i] = R::add(h, d);
+        if (lo[i] != lo[i]) lo[i] = R::neg(inf);              // (an overflow: the whole axis)
+        if (hi[i] != hi[i]) hi[i] = inf;
+        mid[i] = R::mul(R::add(lo[i], hi[i]), T(0.5));
+        if (!R::is_finite(mid[i])) mid[i] = T(0);
+        if (!ok) { lo[i] = inf; hi[i] = R::neg(inf); mid[i] = T(0); }
+    }
+    box.min.x = lo[0]; box.min.y = lo[1]; box.min.z = lo[2];
+    box.max.x = hi[0]; box.max.y = hi[1]; box.max.z = hi[2];
+    centre.x = mid[0]; centre.y = mid[1]; centre.z = mid[2];
+}
+
+// The triangle leaf of trace_instances (both builds): the library's leaf_range over [first, first + count) of instance
+// `inst`'s bottom tree, without its own tie rule (a slot of another bottom tree is not comparable through this tree's
+// prim_ids).  The filter applies the canonical rule on (instance, original id) instead, then the shader's accept, and
+// notes the instance of an accepted hit.
+template <typename T, bool TieLastVisited, typename Shader, typename Payload>
+BVH_HD void instance_leaf(const Shader& shader, const bvhb200::DevTri<T>* tris, const uint32_t* ids, uint32_t inst, Payload& payload,
+                          uint32_t first, uint32_t count, bvhb200::RayCtx<T>& r, bvhb200::HitState<T>& hit, uint32_t& hit_inst) {
+    bvhb200::leaf_range<T>(tris, ids, false, first, count, r, hit, nullptr, [&](uint32_t slot, T t, T u, T v) {
+        const uint32_t id = ids[slot];
+        if (!TieLastVisited && hit.slot != bvhb200::kInvalidId && !(t < hit.t)) {      // an exact tie with the current best
+            if (inst != hit_inst ? inst > hit_inst : !(id < ids[hit.slot])) return false;
+        }
+        if (!static_cast<bool>(shader.accept(payload, inst, static_cast<size_t>(id), t, u, v))) return false;
+        hit_inst = inst;
+        return true;
+    });
 }
 }
 
@@ -798,6 +998,133 @@ device_view_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned 
     bvhb200::run_rounds<false>(run, has_path, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
                                [] {});
 }
+
+// The kernel of DeviceView::trace_instances: device_view_triangle_kernel's scheduler, launch settings and phases, with
+// both levels in one stack machine on the lane's shared-memory stack.  `inst` is the instance the lane is in
+// (kNoInstance at the top level); the inner phase steps through the top tree's nodes or that instance's.  In the leaf
+// phase a top-level leaf enters its first instance: the rest of the leaf (a top-level leaf index), the world ray's
+// origin and direction and the marker are pushed, and the lane's RayCtx becomes the object-space ray with the current
+// tmax.  The bottom traversal then runs in the ordinary inner and leaf phases until it pops the marker (its stack is
+// empty); the leaf phase then pops the world ray back, keeping the shrunk tmax, and goes on with the next entry.
+template <typename T, bool IsAnyHit, bool IsRobust, bool TieLastVisited, typename Shader>
+__global__ void __launch_bounds__(bvhb200::kTraceBlock, sizeof(T) == 4 ? BVH_TRACE_BLOCKS : 4)
+device_view_instance_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned long long n, unsigned long long* cursor,
+                            uint32_t run_rays, uint32_t refill_min, uint32_t inner_budget, detail::InstanceShader<T, Shader> is) {
+    using U = typename bvhb200::Real<T>::UInt;
+    using R = bvhb200::Real<T>;
+    using Payload = typename Shader::Payload;
+    extern __shared__ __align__(128) unsigned char device_view_instance_smem[];
+    constexpr unsigned kFull = 0xFFFFFFFFu;
+    constexpr U kMarker = detail::kInstanceMarker<U>;
+    constexpr U kDone = bvhb200::kTraversalDone<U>;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    bvhb200::SmemStack<U> stack { reinterpret_cast<U*>(device_view_instance_smem) + threadIdx.x, bvhb200::kTraceBlock, 0 };
+
+    bvhb200::RunCursor run;
+    bool has_ray = false;
+    unsigned long long index = 0;
+    bvhb200::RayCtx<T> r;               // the world ray, or inside an instance its object-space ray
+    bvhb200::HitState<T> hit;           // hit.slot is a slot of instance hit_inst's bottom tree
+    uint32_t hit_inst = detail::kNoInstance;
+    uint32_t inst = detail::kNoInstance;
+    Payload payload;
+    U top = 0;
+    auto retire = [&] {
+        const uint32_t* ids = hit_inst != detail::kNoInstance ? is.records[hit_inst].prim_ids : is.prim_ids;
+        is.shader.finish(static_cast<size_t>(index), static_cast<const Payload&>(payload),
+                         detail::make_hit<T>(bvhb200::make_record(hit, hit.t, ids)), hit_inst);
+        has_ray = false;
+    };
+
+    // one draw: the idle lanes take the next rays of the warp's run; a ray whose interval is a NaN retires at once as a miss
+    auto draw = [&] (unsigned idle, unsigned rank) {
+        return detail::draw_run(run, cursor, n, run_rays, lane, has_ray, idle, rank, [&] (unsigned long long i) {
+            index = i;
+            detail::load_ray<T>(is.shader.start(static_cast<size_t>(index), payload), r);
+            hit.slot = bvhb200::kInvalidId; hit.t = r.tmax; hit.u = T(0); hit.v = T(0);
+            hit_inst = detail::kNoInstance;
+            if (bvhb200::ray_interval_is_nan(r)) { retire(); return; }
+            bvhb200::ray_prologue<T, IsRobust>(r);
+            inst = detail::kNoInstance;
+            top = nodes[1].index;
+            stack.clear();
+            has_ray = true;
+        });
+    };
+
+    // inner phase: descend the current level until this lane holds a leaf or the marker, its ray is finished, or the step
+    // budget of this round is spent
+    auto inner = [&] {
+        if (has_ray) {
+            const bvhb200::DevNode<T>* level = inst == detail::kNoInstance ? nodes : is.records[inst].nodes;
+            uint32_t budget = inner_budget;
+            while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone and the marker end it too)
+                --budget;
+                bvhb200::inner_step<T, IsAnyHit, IsRobust>(level, r, top, stack);
+            }
+            if (top == kDone) retire();
+        }
+    };
+
+    // the marker was popped: the world ray back, with the current tmax, and the next entry of the top level
+    auto leave = [&] {
+        for (int k = 2; k >= 0; --k) r.dir[k] = R::from_bits(stack.pop());
+        for (int k = 2; k >= 0; --k) r.org[k] = R::from_bits(stack.pop());
+        bvhb200::ray_prologue<T, IsRobust>(r);
+        inst = detail::kNoInstance;
+        top = bvhb200::pop_or_done<U>(stack);
+    };
+    // `top` is a leaf of the top tree: enter its first instance, or go past it when it is singular
+    auto enter = [&] {
+        const U first = bvhb200::index_first(top);
+        const uint32_t count = bvhb200::index_count(top);
+        const uint32_t id = is.prim_ids[first];
+        const Instance<T>* rec = is.records + id;
+        const U rest = bvhb200::make_index<U>(first + 1, count - 1);
+        if (detail::instance_is_singular(rec->world_to_object)) {
+            top = count > 1 ? rest : bvhb200::pop_or_done<U>(stack);
+            return;
+        }
+        if (count > 1) stack.push(rest);
+        for (int k = 0; k < 3; ++k) stack.push(R::bits(r.org[k]));
+        for (int k = 0; k < 3; ++k) stack.push(R::bits(r.dir[k]));
+        stack.push(kMarker);
+        detail::object_ray(rec->world_to_object, r, r);
+        bvhb200::ray_prologue<T, IsRobust>(r);
+        inst = id;
+        top = rec->root_index;
+    };
+
+    // leaf phase: a bottom leaf's triangles through the filter (the ray ends on an any-hit hit), then the level changes
+    // the next entry asks for, until the lane holds a node of some tree; the ray ends when the top level's stack is empty
+    auto leaf = [&] {
+        if (!has_ray || bvhb200::index_count(top) == 0) return;
+        if (inst != detail::kNoInstance && top != kMarker) {
+            const Instance<T>* rec = is.records + inst;
+            detail::instance_leaf<T, TieLastVisited>(is.shader, rec->tris, rec->prim_ids, inst, payload, (uint32_t)bvhb200::index_first(top),
+                                                     bvhb200::index_count(top), r, hit, hit_inst);
+            if (IsAnyHit && hit.slot != bvhb200::kInvalidId) { retire(); return; }
+            top = bvhb200::pop_or_done<U>(stack);                  // (the marker at the latest)
+        }
+        for (;;) {
+            if (top == kMarker) leave();
+            else if (inst == detail::kNoInstance && bvhb200::index_count(top) != 0 && top != kDone) enter();
+            else break;
+        }
+        if (top == kDone) retire();
+    };
+    bvhb200::run_rounds<false>(run, has_ray, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
+                               [] {});
+}
+
+// The kernel of prepare_instances: one thread per instance record.
+template <typename T>
+__global__ void prepare_instances_kernel(Instance<T>* records, size_t count, typename detail::ViewTypes<T>::BBox* bboxes,
+                                         typename detail::ViewTypes<T>::Vec* centers) {
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i < count) detail::prepare_instance<T>(records[i], bboxes[i], centers[i]);
+}
 #endif
 
 // A plain-data view of one device tree (what bvhNN_get_device_view reports), passed to kernels by value.
@@ -1063,6 +1390,40 @@ template <typename T> struct DeviceView {
 #endif
     }
 
+    // A whole batch of triangle rays through a top-level tree of placed meshes: see "Instanced scenes" at the top of this
+    // file.  This view is the top tree; its primitive k is instances.records[prim_ids[k]].  The workspace is the warps'
+    // run cursor, trace_workspace_bytes() bytes.
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instances(size_t n, const Instances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes) const {
+        trace_instances<IsAnyHit, IsRobust, TieLastVisited>(n, instances, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instances(size_t n, const Instances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes,
+                         void* on_stream) const {
+        if (instances.count != prim_count || (instances.count && !instances.records))
+            throw std::invalid_argument("bvh::v2::cuda::DeviceView::trace_instances: " + std::to_string(instances.count) +
+                                        " instance records for a top tree of " + std::to_string(prim_count) + " primitives");
+        const bvhb200::TracePlan plan = batch_plan<IsAnyHit, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
+        const detail::InstanceShader<T, Shader> is { shader, instances.records, prim_ids };
+        const size_t extra = instances.max_depth + detail::kInstanceStackExtra;
+#if defined(__CUDACC__)
+        run_batch("trace_instances", device_view_instance_kernel<T, IsAnyHit, IsRobust, TieLastVisited, Shader>, is, n, plan.refill_min,
+                  plan.inner_budget, workspace, workspace_bytes, on_stream, extra);
+#else
+        (void)on_stream; (void)plan;
+        batch_stack_bytes("trace_instances", workspace, workspace_bytes, extra);
+        using Payload = typename Shader::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            const Ray ray = shader.start(i, payload);
+            uint32_t hit_inst = detail::kNoInstance;
+            const Hit hit = host_instance_ray<IsAnyHit, IsRobust, TieLastVisited>(is, payload, ray, hit_inst);
+            shader.finish(i, static_cast<const Payload&>(payload), hit, hit_inst);
+        }
+#endif
+    }
+
     // PrecomputedTri::intersect (reference tri.h:55-74) on BVH-order triangle k: true, with the hit's distance and
     // barycentrics, when the ray meets it at a distance in [ray.tmin, ray.tmax].  The batched kernels' own test.
     BVH_HD bool intersect_tri(size_t k, const Ray& ray, T& t, T& u, T& v) const {
@@ -1114,31 +1475,84 @@ private:
         return detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, prim_ids));
     }
 
-    // The checks of trace, query, trace_triangles and trace_paths (`call`): the workspace, then the shared-memory stack of the batched kernels, sized
-    // and bounded as bvhNN_intersect_rays sizes and bounds it.  Returns the stack's bytes per block.
-    size_t batch_stack_bytes(const char* call, void* workspace, size_t workspace_bytes) const {
+    // One ray of trace_instances on the host, the nested loop its contract states: Bvh::intersect on the top tree, whose
+    // leaf enters its instances in BVH order (skipping singular ones), each with the object-space ray, the current tmax, the
+    // bottom tree's Bvh::intersect and the triangle leaf of trace_instances, and carries the shrunk tmax back.  Returns the
+    // record; `hit_inst` is the hit's instance.
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited, typename Shader, typename Payload>
+    Hit host_instance_ray(const detail::InstanceShader<T, Shader>& is, Payload& payload, const Ray& ray, uint32_t& hit_inst) const {
+        bvhb200::RayCtx<T> r;
+        load(ray, r);
+        const T tmax_in = r.tmax;
+        bvhb200::HitState<T> hit { bvhb200::kInvalidId, r.tmax, T(0), T(0) };
+        hit_inst = detail::kNoInstance;
+        if (!bvhb200::ray_interval_is_nan(r)) {
+            bvhb200::ray_prologue<T, IsRobust>(r);
+            detail::VectorStack<Index> stack;
+            stack.elems.reserve(stack_bound());
+            bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
+                nodes, r, root_index(), stack,
+                [&](Index begin, Index end) {
+                    for (Index k = begin; k < end; ++k) {
+                        const uint32_t id = prim_ids[k];
+                        const Instance<T>& rec = is.records[id];
+                        if (detail::instance_is_singular(rec.world_to_object)) continue;
+                        bvhb200::RayCtx<T> o;
+                        detail::object_ray(rec.world_to_object, r, o);
+                        bvhb200::ray_prologue<T, IsRobust>(o);
+                        detail::VectorStack<Index> bottom;
+                        bottom.elems.reserve(rec.depth + 1);
+                        bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
+                            rec.nodes, o, rec.root_index, bottom,
+                            [&](Index b, Index e) {
+                                detail::instance_leaf<T, TieLastVisited>(is.shader, rec.tris, rec.prim_ids, id, payload, (uint32_t)b,
+                                                                         (uint32_t)(e - b), o, hit, hit_inst);
+                                return hit.slot != bvhb200::kInvalidId;
+                            },
+                            [](Index) {});
+                        r.tmax = o.tmax;
+                        if (IsAnyHit && hit.slot != bvhb200::kInvalidId) return true;
+                    }
+                    return hit.slot != bvhb200::kInvalidId;
+                },
+                [](Index) {});
+        }
+        const uint32_t* ids = hit_inst != detail::kNoInstance ? is.records[hit_inst].prim_ids : prim_ids;
+        return detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, ids));
+    }
+
+    // The checks of trace, query, trace_triangles, trace_paths and trace_instances (`call`): the workspace, then the
+    // shared-memory stack of the batched kernels, sized and bounded as bvhNN_intersect_rays sizes and bounds it, with
+    // `extra` entries per thread beyond the tree's own (trace_instances: the bottom trees' and an instance visit's).
+    // Returns the stack's bytes per block.
+    size_t batch_stack_bytes(const char* call, void* workspace, size_t workspace_bytes, size_t extra = 0) const {
         const std::string who = std::string("bvh::v2::cuda::DeviceView::") + call;
         const size_t need = trace_workspace_bytes();
         if (workspace_bytes < need || !workspace)
             throw std::length_error(who + ": a workspace of " + std::to_string(workspace ? workspace_bytes : 0) + " bytes is too small (" +
                                     std::to_string(need) + " bytes)");
-        const size_t smem = (size_t)bvhb200::stack_entries(static_cast<uint32_t>(depth), bvhb200::kDefaultStackRound) *
-                            bvhb200::kTraceBlock * sizeof(Index);
+        const size_t entries = depth + extra;
+        const size_t smem = entries > kMaxTraceSmem ? kMaxTraceSmem + 1             // (too deep for any stack: no overflow below)
+                                                    : (size_t)bvhb200::stack_entries(static_cast<uint32_t>(entries), bvhb200::kDefaultStackRound) *
+                                                          bvhb200::kTraceBlock * sizeof(Index);
         if (smem > kMaxTraceSmem)
-            throw std::length_error(who + ": a tree of depth " + std::to_string(depth) + " needs " + std::to_string(smem) +
-                                    " bytes of shared-memory stack per block, more than " + std::to_string(kMaxTraceSmem));
+            throw std::length_error(who + ": a tree of depth " + std::to_string(depth) +
+                                    (extra ? " with " + std::to_string(extra) + " more entries per ray for its instances" : std::string()) +
+                                    " needs " + std::to_string(smem) + " bytes of shared-memory stack per block, more than " +
+                                    std::to_string(kMaxTraceSmem));
         return smem;
     }
 #if defined(__CUDACC__)
-    // The launch of trace, query, trace_triangles and trace_paths: the checks, then, unless n == 0, the current device
-    // switched to the tree's, the run cursor reset, and one resident wave of `kernel` (device_view_trace_kernel,
-    // device_view_query_kernel, device_view_triangle_kernel or device_view_path_kernel) on `on_stream` with the run length
+    // The launch of trace, query, trace_triangles, trace_paths and trace_instances: the checks, then, unless n == 0, the
+    // current device switched to the tree's, the run cursor reset, and one resident wave of `kernel` (device_view_trace_kernel,
+    // device_view_query_kernel, device_view_triangle_kernel, device_view_path_kernel or device_view_instance_kernel) on `on_stream` with the run length
     // and grid of bvhNN_intersect_rays' persistent kernel.
+    // `extra`: stack entries per thread beyond the tree's own (batch_stack_bytes).
     template <typename Fn>
     void run_batch(const char* call, void (*kernel)(const Node*, unsigned long long, unsigned long long*, uint32_t, uint32_t, uint32_t, Fn),
                    const Fn& fn, size_t n, uint32_t refill_min, uint32_t inner_budget, void* workspace, size_t workspace_bytes,
-                   void* on_stream) const {
-        const size_t smem = batch_stack_bytes(call, workspace, workspace_bytes);
+                   void* on_stream, size_t extra = 0) const {
+        const size_t smem = batch_stack_bytes(call, workspace, workspace_bytes, extra);
         if (n == 0) return;
         cudaStream_t s = static_cast<cudaStream_t>(on_stream);
         int previous = 0;
@@ -1171,5 +1585,45 @@ private:
 #endif
     BVH_HD static void load(const Ray& ray, bvhb200::RayCtx<T>& r) { detail::load_ray<T>(ray, r); }
 };
+
+// An instance record of the mesh `view` (which must have triangles) placed by `object_to_world` (12 values, 3 x 4
+// row-major), on the host or the device.  world_to_object is NaN and root_index 0 until prepare_instances writes them.
+template <typename T> BVH_HD Instance<T> make_instance(const DeviceView<T>& view, const T* object_to_world) {
+    using R = bvhb200::Real<T>;
+    Instance<T> rec;
+    rec.nodes = view.nodes; rec.prim_ids = view.prim_ids; rec.tris = view.tris;
+    rec.root_index = 0;                 // (prepare_instances reads it: on the GPU the nodes are not host memory)
+    rec.depth = static_cast<uint32_t>(view.depth);
+    for (int k = 0; k < 12; ++k) {
+        rec.object_to_world[k] = object_to_world[k];
+        rec.world_to_object[k] = R::from_bits(~(typename R::UInt)0 >> 1);
+    }
+    return rec;
+}
+
+// For every record of `instances` (one thread each, stream-ordered on `stream`, no host synchronisation): its
+// root index and world_to_object, and in bboxes[i] / centers[i] (device arrays of instances.count) the world box of its bottom root box
+// and that box's centre, ready for bvhNN_build_boxes or bvhNN_refit_boxes with BVH_DEVICE_POINTERS.  See
+// detail::prepare_instance for the arithmetic and the bound.  A matrix without an inverse gets an empty box, so the top
+// tree never reaches it, and a NaN world_to_object, so trace_instances skips it in a leaf it shares.  The current device
+// must be the records'.  A failed launch throws std::runtime_error.  Compiled as plain host C++, the records are
+// prepared serially in place.
+template <typename T>
+void prepare_instances(const Instances<T>& instances, typename detail::ViewTypes<T>::BBox* bboxes,
+                       typename detail::ViewTypes<T>::Vec* centers, void* stream = nullptr) {
+    if (instances.count == 0) return;
+    if (!instances.records || !bboxes || !centers)
+        throw std::invalid_argument("bvh::v2::cuda::prepare_instances: null records, boxes or centres");
+#if defined(__CUDACC__)
+    const unsigned block = 128, grid = (unsigned)((instances.count + block - 1) / block);
+    prepare_instances_kernel<T><<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(instances.records, instances.count, bboxes, centers);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess)
+        throw std::runtime_error(std::string("bvh::v2::cuda::prepare_instances: launch: ") + cudaGetErrorString(e));
+#else
+    (void)stream;
+    for (size_t i = 0; i < instances.count; ++i) detail::prepare_instance<T>(instances.records[i], bboxes[i], centers[i]);
+#endif
+}
 
 } // namespace bvh::v2::cuda
