@@ -78,6 +78,8 @@ PATH_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_path_trace_kernels.
 PATH_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_path_trace_kernels.so")
 INSTANCE_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_instance_trace_kernels.cu")
 INSTANCE_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_instance_trace_kernels.so")
+INSTANCE_PATH_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_instance_path_trace_kernels.cu")
+INSTANCE_PATH_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_instance_path_trace_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -152,6 +154,14 @@ def build_device_instance_trace_tests(force: bool = False, verbose: bool = False
     recording shader, the same rays nested by hand one thread each, the benchmark's plain shaders and a hand-nested
     DeviceView::trace tracer)."""
     return _build_test_kernels(INSTANCE_TRACE_KERNELS_SRC, INSTANCE_TRACE_KERNELS_LIB, force, verbose)
+
+
+def build_device_instance_path_trace_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_instance_path_trace_kernels.cu: the test shaders of DeviceView::trace_instance_paths (a path tracer
+    with next-event shadow segments over placed meshes, as one call, as a wavefront loop of trace_instances and as
+    trace_paths on one mesh; a recording shader of scripted segments) and the same segments nested by hand one thread
+    each."""
+    return _build_test_kernels(INSTANCE_PATH_TRACE_KERNELS_SRC, INSTANCE_PATH_TRACE_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

@@ -423,6 +423,59 @@
 //     // bvh3f_refit_boxes(top_bvh, d_boxes, 3, BVH_DEVICE_POINTERS) after prepare_instances on the top handle's stream
 //     top.trace_instances<false, false>(n, instances, Shade { d_rays, d_hits, d_inst }, workspace, bytes, stream);
 //
+// Paths through instanced scenes: top.trace_instance_paths<IsRobust, TieLastVisited = false>(n, instances, shader,
+// workspace, workspace_bytes[, stream]) is trace_paths over the two-level scene of trace_instances: `top` and `instances`
+// as for trace_instances, and a shader with a Payload type (per-path state, kept in registers) and four __device__ (or
+// __host__ __device__) functions:
+//     PathStep start(size_t i, Payload& p, Ray& ray) const;                                 // world-space first segment, or End
+//     bool     accept(Payload& p, uint32_t instance, size_t prim_id, T t, T u, T v) const;  // as in trace_instances
+//     PathStep next(size_t i, Payload& p, const Hit& hit, uint32_t instance, Ray& ray) const;
+//     void     finish(size_t i, const Payload& p) const;
+//   * for every i in [0, n), start is called once, then zero or more segments, then finish once.  If start returns End,
+//     finish follows directly;
+//   * a Closest segment is exactly trace_instances<false, IsRobust, TieLastVisited> for that world ray, an Occlusion
+//     segment trace_instances<true, IsRobust, TieLastVisited>: the same accept calls (instance, original id, bits of t, u
+//     and v) in the same order, then next with the record and instance trace_instances' finish would get (kNoInstance,
+//     all ones, on a miss).  A segment whose interval is a NaN gets no accept call and a miss record;
+//   * on entry to next, `ray` is the segment's world ray as start or the previous next returned it, bit for bit: not
+//     shrunk and not in object space.  On a return other than End, `ray` is the next segment;
+//   * the payload lives across segments; lanes of one warp may be in different segment kinds and at different levels;
+//   * one identity instance under a top tree of one leaf gives trace_paths on that mesh bit for bit, instance 0 for every
+//     hit;
+//   * errors, checked on the host before any launch, as for trace_instances: instances.count other than the top tree's
+//     prim_count throws std::invalid_argument; a stack of top depth + max_depth + 9 entries beyond the 200 KB
+//     shared-memory stack, or a small workspace, std::length_error; a failed launch std::runtime_error.  The workspace
+//     (trace_workspace_bytes()), n == 0, streams, the current device, the warp subset and the watchdog are those of
+//     trace_paths.  Compiled as plain host C++, the paths run serially, each segment through the nested loop of one
+//     trace_instances ray.
+// The kernel is bvh::v2::cuda::device_view_instance_path_kernel<T, IsRobust, TieLastVisited, Shader>, with
+// trace_instances' launch bounds, block, stack and launch and plan_trace's closest-hit settings.  A lane's segment kind
+// picks the any-hit or closest-hit inner step at either level.  An occlusion segment can end inside an instance: the
+// world origin and direction are then popped back from under the marker on the lane's stack before next runs.  The
+// payload competes with the traversal for the float kernel's 56 registers.  A shadow-ray shader that skips the
+// (instance, triangle) its path stands on (INTEGRATION.md §5 has a path tracer whole):
+//
+//     struct Paths {
+//         struct Payload { uint32_t inst, prim; float radiance; };
+//         ...                                                                 // camera, light, records, radiance out
+//         __device__ PathStep start(size_t i, Payload& p, bvh_ray3f& ray) const {
+//             ray = camera_ray(i); p = { kNoInstance, UINT32_MAX, 0.0f };
+//             return PathStep::Closest;
+//         }
+//         __device__ bool accept(Payload& p, uint32_t k, size_t id, float, float, float) const { return !(k == p.inst && id == p.prim); }
+//         __device__ PathStep next(size_t i, Payload& p, const bvh_hit3f& hit, uint32_t k, bvh_ray3f& ray) const {
+//             if (p.inst != kNoInstance || hit.prim_id == UINT32_MAX) {   // the shadow segment ended, or a primary miss
+//                 p.radiance = p.inst != kNoInstance && hit.prim_id == UINT32_MAX ? 1.0f : 0.0f;
+//                 return PathStep::End;
+//             }
+//             p.inst = k; p.prim = hit.prim_id;
+//             ray.org = ray.org + hit.t * ray.dir; ray.dir = light - ray.org; ray.tmin = 0.0f; ray.tmax = 1.0f;
+//             return PathStep::Occlusion;
+//         }
+//         __device__ void finish(size_t i, const Payload& p) const { image[i] = p.radiance; }
+//     };
+//     top.trace_instance_paths<false>(width * height, instances, Paths { ... }, workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -700,6 +753,91 @@ __device__ __forceinline__ bool draw_run(bvhb200::RunCursor& run, unsigned long 
     run.pos += take;
     return true;
 }
+
+// The steps the path kernels (device_view_path_kernel, device_view_instance_path_kernel) and the instance kernels
+// (device_view_instance_kernel, device_view_instance_path_kernel) share.  Each kernel keeps a lambda per step that
+// forwards to the helper, and that form compiles the older kernels to the same instructions as when the lambdas held
+// the code.  One step stays in the kernels: the root part of arming a segment (prologue, root index, empty stack).
+// Every helper form tried for it (the whole arm as one helper, with the nodes by value, by reference or through a
+// callable, `inline` or `__forceinline__`, or this part as a helper of its own) reordered device_view_path_kernel's
+// instructions.
+//
+// reset_segment: the first part of arming a lane for its next segment: the ray, its tmax as the shader gave it (r.tmax
+// shrinks on hits), a reset hit state and the segment kind.  The kernel then sets `top` to kTraversalDone for a segment
+// whose interval is a NaN (no traversal: it ends as a miss in the next leaf phase, with no accept call), and otherwise
+// runs the prologue and takes the root, and clears the stack.
+template <typename T, typename Ray>
+__device__ __forceinline__ void reset_segment(PathStep step, const Ray& ray, bvhb200::RayCtx<T>& r, T& tmax_in, bvhb200::HitState<T>& hit,
+                                              bool& occlusion) {
+    load_ray<T>(ray, r);
+    tmax_in = r.tmax;
+    hit.slot = bvhb200::kInvalidId; hit.t = r.tmax; hit.u = T(0); hit.v = T(0);
+    occlusion = step == PathStep::Occlusion;
+}
+// A segment ended: next(ray) receives its ray as the shader gave it (r's origin, direction and tmin, tmax_in) and
+// returns the next step; End retires the path, anything else arms the lane with the ray next left.
+template <typename Ray, typename T, typename Next, typename Retire, typename Arm>
+__device__ __forceinline__ void end_segment(const bvhb200::RayCtx<T>& r, T tmax_in, Next&& next, Retire&& retire, Arm&& arm) {
+    Ray ray = make_ray<Ray>(r);
+    ray.tmax = tmax_in;
+    const PathStep step = next(ray);
+    if (step == PathStep::End) retire();
+    else arm(step, ray);
+}
+
+// The two-level stack machine of DeviceView::trace_instances and trace_instance_paths on a lane's shared-memory stack.
+// `inst` is the instance the lane is in (kNoInstance at the top level), `r` the world ray or inside an instance its
+// object-space ray.  Entering an instance pushes the rest of the top leaf (when it has more), the world ray's origin and
+// direction and the marker, then makes `r` the object-space ray with the current tmax.
+//
+// pop_world_ray: the world ray's origin and direction, from the six entries on top of the stack, into `r`.
+template <typename T, typename U> __device__ __forceinline__ void pop_world_ray(bvhb200::SmemStack<U>& stack, bvhb200::RayCtx<T>& r) {
+    using R = bvhb200::Real<T>;
+    for (int k = 2; k >= 0; --k) r.dir[k] = R::from_bits(stack.pop());
+    for (int k = 2; k >= 0; --k) r.org[k] = R::from_bits(stack.pop());
+}
+// leave_instance: the marker was popped: the world ray back, with the current tmax, and the next entry of the top level
+template <typename T, bool IsRobust, typename U>
+__device__ __forceinline__ void leave_instance(bvhb200::SmemStack<U>& stack, bvhb200::RayCtx<T>& r, uint32_t& inst, U& top) {
+    pop_world_ray<T>(stack, r);
+    bvhb200::ray_prologue<T, IsRobust>(r);
+    inst = kNoInstance;
+    top = bvhb200::pop_or_done<U>(stack);
+}
+// enter_instance: `top` is a leaf of the top tree: enter its first instance, or go past it when it is singular
+template <typename T, bool IsRobust, typename U, typename Shader>
+__device__ __forceinline__ void enter_instance(const InstanceShader<T, Shader>& is, bvhb200::SmemStack<U>& stack, bvhb200::RayCtx<T>& r,
+                                               uint32_t& inst, U& top) {
+    using R = bvhb200::Real<T>;
+    const U first = bvhb200::index_first(top);
+    const uint32_t count = bvhb200::index_count(top);
+    const uint32_t id = is.prim_ids[first];
+    const Instance<T>* rec = is.records + id;
+    const U rest = bvhb200::make_index<U>(first + 1, count - 1);
+    if (instance_is_singular(rec->world_to_object)) {
+        top = count > 1 ? rest : bvhb200::pop_or_done<U>(stack);
+        return;
+    }
+    if (count > 1) stack.push(rest);
+    for (int k = 0; k < 3; ++k) stack.push(R::bits(r.org[k]));
+    for (int k = 0; k < 3; ++k) stack.push(R::bits(r.dir[k]));
+    stack.push(kInstanceMarker<U>);
+    object_ray(rec->world_to_object, r, r);
+    bvhb200::ray_prologue<T, IsRobust>(r);
+    inst = id;
+    top = rec->root_index;
+}
+// walk_levels: the level changes the entry in `top` asks for, until the lane holds a node of some tree (or
+// kTraversalDone: the top level's stack is empty): leave() (leave_instance) on the marker, enter() (enter_instance) on a
+// leaf of the top tree
+template <typename U, typename Leave, typename Enter>
+__device__ __forceinline__ void walk_levels(const U& top, const uint32_t& inst, Leave&& leave, Enter&& enter) {
+    for (;;) {
+        if (top == kInstanceMarker<U>) leave();
+        else if (inst == kNoInstance && bvhb200::index_count(top) != 0 && top != bvhb200::kTraversalDone<U>) enter();
+        else break;
+    }
+}
 }
 
 // The kernel of DeviceView::trace: the library's persistent scheduler (persistent_core.cuh) over the caller's tracer.
@@ -938,10 +1076,7 @@ device_view_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned 
     // the lane's next segment: hit state reset, prologue, root, empty stack.  A segment whose interval is a NaN gets no
     // traversal: it starts at kTraversalDone and ends as a miss in the next leaf phase, with no accept call.
     auto arm = [&](PathStep step, const Ray& ray) {
-        detail::load_ray<T>(ray, r);
-        tmax_in = r.tmax;
-        hit.slot = bvhb200::kInvalidId; hit.t = r.tmax; hit.u = T(0); hit.v = T(0);
-        occlusion = step == PathStep::Occlusion;
+        detail::reset_segment<T>(step, ray, r, tmax_in, hit, occlusion);
         top = bvhb200::kTraversalDone<U>;
         if (!bvhb200::ray_interval_is_nan(r)) {
             bvhb200::ray_prologue<T, IsRobust>(r);
@@ -953,12 +1088,10 @@ device_view_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned 
 
     // a segment ended: its record and its ray as the shader gave it to next, then the next segment or the path's end
     auto end_segment = [&] {
-        Ray ray = detail::make_ray<Ray>(r);
-        ray.tmax = tmax_in;
-        const PathStep step = ts.shader.next(static_cast<size_t>(index), payload,
-                                             detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, ts.prim_ids)), ray);
-        if (step == PathStep::End) retire();
-        else arm(step, ray);
+        detail::end_segment<Ray>(r, tmax_in, [&](Ray& ray) {
+            return ts.shader.next(static_cast<size_t>(index), payload,
+                                  detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, ts.prim_ids)), ray);
+        }, retire, arm);
     };
 
     // one draw: the idle lanes take the next paths of the warp's run
@@ -1011,7 +1144,6 @@ __global__ void __launch_bounds__(bvhb200::kTraceBlock, sizeof(T) == 4 ? BVH_TRA
 device_view_instance_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned long long n, unsigned long long* cursor,
                             uint32_t run_rays, uint32_t refill_min, uint32_t inner_budget, detail::InstanceShader<T, Shader> is) {
     using U = typename bvhb200::Real<T>::UInt;
-    using R = bvhb200::Real<T>;
     using Payload = typename Shader::Payload;
     extern __shared__ __align__(128) unsigned char device_view_instance_smem[];
     constexpr unsigned kFull = 0xFFFFFFFFu;
@@ -1068,33 +1200,9 @@ device_view_instance_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsig
     };
 
     // the marker was popped: the world ray back, with the current tmax, and the next entry of the top level
-    auto leave = [&] {
-        for (int k = 2; k >= 0; --k) r.dir[k] = R::from_bits(stack.pop());
-        for (int k = 2; k >= 0; --k) r.org[k] = R::from_bits(stack.pop());
-        bvhb200::ray_prologue<T, IsRobust>(r);
-        inst = detail::kNoInstance;
-        top = bvhb200::pop_or_done<U>(stack);
-    };
+    auto leave = [&] { detail::leave_instance<T, IsRobust>(stack, r, inst, top); };
     // `top` is a leaf of the top tree: enter its first instance, or go past it when it is singular
-    auto enter = [&] {
-        const U first = bvhb200::index_first(top);
-        const uint32_t count = bvhb200::index_count(top);
-        const uint32_t id = is.prim_ids[first];
-        const Instance<T>* rec = is.records + id;
-        const U rest = bvhb200::make_index<U>(first + 1, count - 1);
-        if (detail::instance_is_singular(rec->world_to_object)) {
-            top = count > 1 ? rest : bvhb200::pop_or_done<U>(stack);
-            return;
-        }
-        if (count > 1) stack.push(rest);
-        for (int k = 0; k < 3; ++k) stack.push(R::bits(r.org[k]));
-        for (int k = 0; k < 3; ++k) stack.push(R::bits(r.dir[k]));
-        stack.push(kMarker);
-        detail::object_ray(rec->world_to_object, r, r);
-        bvhb200::ray_prologue<T, IsRobust>(r);
-        inst = id;
-        top = rec->root_index;
-    };
+    auto enter = [&] { detail::enter_instance<T, IsRobust>(is, stack, r, inst, top); };
 
     // leaf phase: a bottom leaf's triangles through the filter (the ray ends on an any-hit hit), then the level changes
     // the next entry asks for, until the lane holds a node of some tree; the ray ends when the top level's stack is empty
@@ -1107,14 +1215,121 @@ device_view_instance_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsig
             if (IsAnyHit && hit.slot != bvhb200::kInvalidId) { retire(); return; }
             top = bvhb200::pop_or_done<U>(stack);                  // (the marker at the latest)
         }
-        for (;;) {
-            if (top == kMarker) leave();
-            else if (inst == detail::kNoInstance && bvhb200::index_count(top) != 0 && top != kDone) enter();
-            else break;
-        }
+        detail::walk_levels(top, inst, leave, enter);
         if (top == kDone) retire();
     };
     bvhb200::run_rounds<false>(run, has_ray, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
+                               [] {});
+}
+
+// The kernel of DeviceView::trace_instance_paths: device_view_instance_kernel's scheduler, launch settings and two-level
+// stack machine, with a path per lane as in device_view_path_kernel.  Each segment steps through the current level with
+// the any-hit or closest-hit inner step by the lane's segment kind.  A segment ends in the leaf phase, on an accepted
+// occlusion hit or when the top level is done; an occlusion hit can end it inside an instance, and then the world ray's
+// origin and direction are popped back from under the marker before next sees the ray.  next receives the record and
+// the hit's instance, and the lane re-arms at the top level or retires the path.
+template <typename T, bool IsRobust, bool TieLastVisited, typename Shader>
+__global__ void __launch_bounds__(bvhb200::kTraceBlock, sizeof(T) == 4 ? BVH_TRACE_BLOCKS : 4)
+device_view_instance_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned long long n, unsigned long long* cursor,
+                                 uint32_t run_rays, uint32_t refill_min, uint32_t inner_budget, detail::InstanceShader<T, Shader> is) {
+    using U = typename bvhb200::Real<T>::UInt;
+    using Payload = typename Shader::Payload;
+    using Ray = typename detail::ViewTypes<T>::Ray;
+    extern __shared__ __align__(128) unsigned char device_view_instance_path_smem[];
+    constexpr unsigned kFull = 0xFFFFFFFFu;
+    constexpr U kMarker = detail::kInstanceMarker<U>;
+    constexpr U kDone = bvhb200::kTraversalDone<U>;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    bvhb200::SmemStack<U> stack { reinterpret_cast<U*>(device_view_instance_path_smem) + threadIdx.x, bvhb200::kTraceBlock, 0 };
+
+    bvhb200::RunCursor run;
+    bool has_path = false;
+    unsigned long long index = 0;
+    bvhb200::RayCtx<T> r;               // the world ray, or inside an instance its object-space ray
+    bvhb200::HitState<T> hit;           // hit.slot is a slot of instance hit_inst's bottom tree
+    uint32_t hit_inst = detail::kNoInstance;
+    uint32_t inst = detail::kNoInstance;
+    T tmax_in = T(0);                   // the segment's tmax as the shader gave it
+    bool occlusion = false;             // the segment's kind
+    Payload payload;
+    U top = 0;
+    auto retire = [&] {
+        is.shader.finish(static_cast<size_t>(index), static_cast<const Payload&>(payload));
+        has_path = false;
+    };
+
+    // the lane's next segment, at the top level: device_view_path_kernel's arm, and no instance
+    auto arm = [&](PathStep step, const Ray& ray) {
+        detail::reset_segment<T>(step, ray, r, tmax_in, hit, occlusion);
+        top = bvhb200::kTraversalDone<U>;
+        if (!bvhb200::ray_interval_is_nan(r)) {
+            bvhb200::ray_prologue<T, IsRobust>(r);
+            top = nodes[1].index;
+        }
+        stack.clear();
+        hit_inst = detail::kNoInstance;
+        inst = detail::kNoInstance;
+        has_path = true;
+    };
+
+    // a segment ended: inside an instance (an occlusion hit) the world ray comes back from under the marker; then its
+    // record, instance and world ray to next, and the next segment or the path's end
+    auto end_segment = [&] {
+        if (inst != detail::kNoInstance) {
+            while (stack.pop() != kMarker) {}
+            detail::pop_world_ray<T>(stack, r);
+        }
+        detail::end_segment<Ray>(r, tmax_in, [&](Ray& ray) {
+            const uint32_t* ids = hit_inst != detail::kNoInstance ? is.records[hit_inst].prim_ids : is.prim_ids;
+            return is.shader.next(static_cast<size_t>(index), payload, detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, ids)),
+                                  hit_inst, ray);
+        }, retire, arm);
+    };
+
+    // one draw: the idle lanes take the next paths of the warp's run
+    auto draw = [&] (unsigned idle, unsigned rank) {
+        return detail::draw_run(run, cursor, n, run_rays, lane, has_path, idle, rank, [&] (unsigned long long i) {
+            index = i;
+            Ray ray;
+            const PathStep step = is.shader.start(static_cast<size_t>(index), payload, ray);
+            if (step == PathStep::End) retire();
+            else arm(step, ray);
+        });
+    };
+
+    // inner phase: descend the current level until this lane holds a leaf or the marker, its segment is finished, or the
+    // step budget of this round is spent
+    auto inner = [&] {
+        if (has_path) {
+            const bvhb200::DevNode<T>* level = inst == detail::kNoInstance ? nodes : is.records[inst].nodes;
+            uint32_t budget = inner_budget;
+            while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone and the marker end it too)
+                --budget;
+                if (occlusion) bvhb200::inner_step<T, true, IsRobust>(level, r, top, stack);
+                else bvhb200::inner_step<T, false, IsRobust>(level, r, top, stack);
+            }
+        }
+    };
+
+    auto leave = [&] { detail::leave_instance<T, IsRobust>(stack, r, inst, top); };
+    auto enter = [&] { detail::enter_instance<T, IsRobust>(is, stack, r, inst, top); };
+
+    // leaf phase: a bottom leaf's triangles through the filter, then the level walk of device_view_instance_kernel; the
+    // segment ends on an occlusion hit or when the top level is done (kTraversalDone, also a NaN segment's start)
+    auto leaf = [&] {
+        if (!has_path || bvhb200::index_count(top) == 0) return;
+        if (inst != detail::kNoInstance && top != kMarker) {
+            const Instance<T>* rec = is.records + inst;
+            detail::instance_leaf<T, TieLastVisited>(is.shader, rec->tris, rec->prim_ids, inst, payload, (uint32_t)bvhb200::index_first(top),
+                                                     bvhb200::index_count(top), r, hit, hit_inst);
+            if (occlusion && hit.slot != bvhb200::kInvalidId) { end_segment(); return; }
+            top = bvhb200::pop_or_done<U>(stack);                  // (the marker at the latest)
+        }
+        detail::walk_levels(top, inst, leave, enter);
+        if (top == kDone) end_segment();
+    };
+    bvhb200::run_rounds<false>(run, has_path, kFull, 0u, 0u, nullptr, kFull, refill_min, lt_mask, lane, draw, [] {}, inner, leaf,
                                [] {});
 }
 
@@ -1424,6 +1639,45 @@ template <typename T> struct DeviceView {
 #endif
     }
 
+    // Whole paths through a top-level tree of placed meshes, each segment continued in place from the last: see "Paths
+    // through instanced scenes" at the top of this file.  This view is the top tree, as for trace_instances.  The
+    // workspace is the warps' run cursor, trace_workspace_bytes() bytes.
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instance_paths(size_t n, const Instances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes) const {
+        trace_instance_paths<IsRobust, TieLastVisited>(n, instances, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instance_paths(size_t n, const Instances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes,
+                              void* on_stream) const {
+        if (instances.count != prim_count || (instances.count && !instances.records))
+            throw std::invalid_argument("bvh::v2::cuda::DeviceView::trace_instance_paths: " + std::to_string(instances.count) +
+                                        " instance records for a top tree of " + std::to_string(prim_count) + " primitives");
+        const bvhb200::TracePlan plan = batch_plan<false, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
+        const detail::InstanceShader<T, Shader> is { shader, instances.records, prim_ids };
+        const size_t extra = instances.max_depth + detail::kInstanceStackExtra;
+#if defined(__CUDACC__)
+        run_batch("trace_instance_paths", device_view_instance_path_kernel<T, IsRobust, TieLastVisited, Shader>, is, n, plan.refill_min,
+                  plan.inner_budget, workspace, workspace_bytes, on_stream, extra);
+#else
+        (void)on_stream; (void)plan;
+        batch_stack_bytes("trace_instance_paths", workspace, workspace_bytes, extra);
+        using Payload = typename Shader::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            Ray ray;
+            PathStep step = shader.start(i, payload, ray);
+            while (step != PathStep::End) {
+                uint32_t hit_inst = detail::kNoInstance;
+                const Hit hit = step == PathStep::Occlusion ? host_instance_ray<true, IsRobust, TieLastVisited>(is, payload, ray, hit_inst)
+                                                            : host_instance_ray<false, IsRobust, TieLastVisited>(is, payload, ray, hit_inst);
+                step = shader.next(i, payload, hit, hit_inst, ray);
+            }
+            shader.finish(i, static_cast<const Payload&>(payload));
+        }
+#endif
+    }
+
     // PrecomputedTri::intersect (reference tri.h:55-74) on BVH-order triangle k: true, with the hit's distance and
     // barycentrics, when the ray meets it at a distance in [ray.tmin, ray.tmax].  The batched kernels' own test.
     BVH_HD bool intersect_tri(size_t k, const Ray& ray, T& t, T& u, T& v) const {
@@ -1441,7 +1695,8 @@ private:
     // the shared memory a persistent block may have, as bvhNN_intersect_rays bounds it
     static constexpr size_t kMaxTraceSmem = 200 * 1024;
 
-    // The library's scheduling of a persistent closest-hit or any-hit batch (trace, trace_triangles, trace_paths), with its default
+    // The library's scheduling of a persistent closest-hit or any-hit batch (trace, trace_triangles, trace_paths,
+    // trace_instances, trace_instance_paths), with its default
     // settings; `flags` adds kTraceLastVisited.
     template <bool IsAnyHit, bool IsRobust> static bvhb200::TracePlan batch_plan(size_t n, unsigned flags) {
         bvhb200::TraceRequest request {};
@@ -1521,9 +1776,10 @@ private:
         return detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, ids));
     }
 
-    // The checks of trace, query, trace_triangles, trace_paths and trace_instances (`call`): the workspace, then the
-    // shared-memory stack of the batched kernels, sized and bounded as bvhNN_intersect_rays sizes and bounds it, with
-    // `extra` entries per thread beyond the tree's own (trace_instances: the bottom trees' and an instance visit's).
+    // The checks of trace, query, trace_triangles, trace_paths, trace_instances and trace_instance_paths (`call`): the
+    // workspace, then the shared-memory stack of the batched kernels, sized and bounded as bvhNN_intersect_rays sizes and
+    // bounds it, with `extra` entries per thread beyond the tree's own (trace_instances and trace_instance_paths: the
+    // bottom trees' and an instance visit's).
     // Returns the stack's bytes per block.
     size_t batch_stack_bytes(const char* call, void* workspace, size_t workspace_bytes, size_t extra = 0) const {
         const std::string who = std::string("bvh::v2::cuda::DeviceView::") + call;
@@ -1543,10 +1799,11 @@ private:
         return smem;
     }
 #if defined(__CUDACC__)
-    // The launch of trace, query, trace_triangles, trace_paths and trace_instances: the checks, then, unless n == 0, the
-    // current device switched to the tree's, the run cursor reset, and one resident wave of `kernel` (device_view_trace_kernel,
-    // device_view_query_kernel, device_view_triangle_kernel, device_view_path_kernel or device_view_instance_kernel) on `on_stream` with the run length
-    // and grid of bvhNN_intersect_rays' persistent kernel.
+    // The launch of trace, query, trace_triangles, trace_paths, trace_instances and trace_instance_paths: the checks, then,
+    // unless n == 0, the current device switched to the tree's, the run cursor reset, and one resident wave of `kernel`
+    // (device_view_trace_kernel, device_view_query_kernel, device_view_triangle_kernel, device_view_path_kernel,
+    // device_view_instance_kernel or device_view_instance_path_kernel) on `on_stream` with the run length and grid of
+    // bvhNN_intersect_rays' persistent kernel.
     // `extra`: stack entries per thread beyond the tree's own (batch_stack_bytes).
     template <typename Fn>
     void run_batch(const char* call, void (*kernel)(const Node*, unsigned long long, unsigned long long*, uint32_t, uint32_t, uint32_t, Fn),
