@@ -80,6 +80,8 @@ INSTANCE_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_instance_trace_
 INSTANCE_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_instance_trace_kernels.so")
 INSTANCE_PATH_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_instance_path_trace_kernels.cu")
 INSTANCE_PATH_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_instance_path_trace_kernels.so")
+MOTION_INSTANCE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_motion_instance_kernels.cu")
+MOTION_INSTANCE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_motion_instance_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -162,6 +164,14 @@ def build_device_instance_path_trace_tests(force: bool = False, verbose: bool = 
     trace_paths on one mesh; a recording shader of scripted segments) and the same segments nested by hand one thread
     each."""
     return _build_test_kernels(INSTANCE_PATH_TRACE_KERNELS_SRC, INSTANCE_PATH_TRACE_KERNELS_LIB, force, verbose)
+
+
+def build_device_motion_instance_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_motion_instance_kernels.cu: the test shaders of the motion forms of DeviceView::trace_instances and
+    trace_instance_paths, prepare_motion_instances and instance_at (a recording shader with a time per ray, the same
+    rays nested by hand one thread each, a path tracer with a time per path as one call and as a wavefront loop, the
+    benchmark's plain shader)."""
+    return _build_test_kernels(MOTION_INSTANCE_KERNELS_SRC, MOTION_INSTANCE_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

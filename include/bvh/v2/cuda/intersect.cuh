@@ -476,6 +476,46 @@
 //     };
 //     top.trace_instance_paths<false>(width * height, instances, Paths { ... }, workspace, bytes, stream);
 //
+// Motion blur: placements that move over the shutter.  A MotionInstance<T> record (make_motion_instance(view, key0,
+// key1)) holds a bottom tree as Instance<T> does and two 3 x 4 keys, object_to_world[0] at time 0 and
+// object_to_world[1] at time 1, and no inverse; MotionInstances<T> { records, count, max_depth } views them.  A ray at
+// time tau sees record k as instance_at(records[k], tau): each coefficient blended linearly, (1 - tau) key0 + tau key1
+// rounded step by step with no FMA, tau clamped to [0, 1] (a NaN time as 0), exact at 0 and 1 and wherever the keys
+// agree; its world_to_object is prepare_instance's inverse of that (detail::blend_keys, detail::invert_affine).
+// prepare_motion_instances(instances, bboxes, centers[, stream]) writes every root index and a world box that holds the
+// record's bottom root box at every time of the shutter (the union of the boxes at the two keys, widened for the
+// rounding of the blend), for bvhNN_build_boxes / bvhNN_refit_boxes, in one stream-ordered kernel.  A key with a
+// non-finite entry gives the empty box; a key without an inverse does not (an object may scale from 0): a ray at a time
+// where the placement has no inverse skips the record.  On the top view:
+//     top.trace_instances<IsAnyHit, IsRobust, TieLastVisited = false>(n, motion_instances, shader, workspace, bytes[, stream]);
+//     top.trace_instance_paths<IsRobust, TieLastVisited = false>(n, motion_instances, shader, workspace, bytes[, stream]);
+// take the shaders of the static calls, except that start also gives the ray's (path's) time:
+//     Ray      start(size_t i, Payload& p, T& time) const;                     // trace_instances
+//     PathStep start(size_t i, Payload& p, Ray& ray, T& time) const;           // trace_instance_paths: for every segment
+//   * per ray (segment), the calls are exactly those of the static call on the same top tree with record k replaced by
+//     instance_at(records[k], time): the same accept calls (instance, original id, bits of t, u, v), record, instance
+//     and, for paths, world ray to next.  With equal keys the motion call is the static call bit for bit at any time;
+//   * errors, workspace, streams, n == 0 and the host build are those of the static calls, the errors naming
+//     "trace_instances (motion)" or "trace_instance_paths (motion)".  Compiled as plain host C++, each ray runs the
+//     nested loop over instance_at;
+//   * the time is kept beside the payload in the lane's registers; each instance entry builds the placement (about 60
+//     multiplies and adds and 9 divisions).  Linear blending of matrices shrinks an object that turns far within one
+//     shutter (a half turn passes through a singular matrix): split such a shutter, or keep the turn small.
+// One frame of a renderer (the keys of frame f are the placements at its shutter's open and close):
+//
+//     struct Shade {
+//         struct Payload {};
+//         const bvh_ray3f* rays; const float* times; bvh_hit3f* hits; uint32_t* inst;
+//         __device__ bvh_ray3f start(size_t i, Payload&, float& time) const { time = times[i]; return rays[i]; }
+//         __device__ bool accept(Payload&, uint32_t, size_t, float, float, float) const { return true; }
+//         __device__ void finish(size_t i, const Payload&, const bvh_hit3f& h, uint32_t k) const { hits[i] = h; inst[i] = k; }
+//     };
+//     write_keys<<<...>>>(d_recs, open, close);                       // yours: records[k].object_to_world[0] and [1]
+//     const MotionInstances<float> instances { d_recs, count, max_depth };
+//     prepare_motion_instances(instances, d_boxes, d_centres, stream);
+//     bvh3f_refit_boxes(top_bvh, d_boxes, count, BVH_DEVICE_POINTERS);    // on the top handle's stream
+//     top.trace_instances<false, false>(n, instances, Shade { d_rays, d_times, d_hits, d_inst }, workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -523,6 +563,27 @@ template <typename T> struct alignas(16) Instance {
 // host sizes the shared-memory stack of trace_instances from it.
 template <typename T> struct Instances {
     Instance<T>* records = nullptr;
+    size_t count = 0;
+    size_t max_depth = 0;
+};
+
+// One placed copy of a triangle mesh that moves over the shutter, for the motion forms of trace_instances and
+// trace_instance_paths: the bottom tree as in Instance<T>, and two placements (keys), object_to_world[0] at time 0 and
+// object_to_world[1] at time 1, each 3 x 4 row-major as in Instance<T>.  A ray at time tau sees the record as
+// instance_at(record, tau).  Fill it with make_motion_instance(view, key0, key1); root_index is written by
+// prepare_motion_instances.  It stores no inverse: the placement at the ray's time is built on every entry.
+template <typename T> struct alignas(16) MotionInstance {
+    const bvhb200::DevNode<T>* nodes;   // the bottom view's nodes, prim_ids (BVH order) and tris (BVH order)
+    const uint32_t* prim_ids;
+    const bvhb200::DevTri<T>* tris;
+    typename bvhb200::Real<T>::UInt root_index;     // the bottom root's index, written by prepare_motion_instances
+    uint32_t depth;                     // the bottom tree's depth
+    T object_to_world[2][12];           // the keys at time 0 and time 1, each row i = A[i][0..2], b[i]
+};
+
+// A plain view of `count` motion records in device memory; max_depth as in Instances<T>.
+template <typename T> struct MotionInstances {
+    MotionInstance<T>* records = nullptr;
     size_t count = 0;
     size_t max_depth = 0;
 };
@@ -599,11 +660,18 @@ BVH_HD void shader_leaf(const TriangleShader<T, Shader>& ts, Payload& payload, u
                            });
 }
 
+// The shader the motion forms of trace_instances and trace_instance_paths run: the caller's, with the ray's time kept
+// beside its payload (so in the lane's registers) from start on; defined below.
+template <typename T, typename Shader> struct MotionShader;
+// The record kind of a shader: Instance<T>, or MotionInstance<T> under a MotionShader.
+template <typename T, typename Shader> struct RecordOf { using type = Instance<T>; };
+template <typename T, typename Shader> struct RecordOf<T, MotionShader<T, Shader>> { using type = MotionInstance<T>; };
+
 // What the kernel of DeviceView::trace_instances reads besides the top tree's nodes: the caller's shader, the instance
 // records and the top tree's prim_ids (BVH-order slot -> record).
 template <typename T, typename Shader> struct InstanceShader {
     Shader shader;
-    const Instance<T>* records;
+    const typename RecordOf<T, Shader>::type* records;
     const uint32_t* prim_ids;
 };
 // The instance trace_instances reports for a miss
@@ -640,20 +708,13 @@ template <typename T> BVH_HD void object_ray(const T* world_to_object, const bvh
 // An instance trace_instances skips: prepare_instances found no inverse (its world_to_object is NaN)
 template <typename T> BVH_HD bool instance_is_singular(const T* world_to_object) { return world_to_object[0] != world_to_object[0]; }
 
-// prepare_instances for one record (both builds).  root_index: the bottom root's.  world_to_object: the adjugate of A over its determinant, then
-// -(A^-1 b); all NaN when an entry of object_to_world is not finite, the determinant is 0 or not finite, or an entry of
-// the inverse is not finite.  The world box of the bottom root box [lo, hi]: per axis i, b_i plus the sums of
-// min / max(a_ij lo_j, a_ij hi_j), which in exact arithmetic is the box of the eight transformed corners.  Its rounding
-// error is below 2.5 eps S_i, S_i = |b_i| + sum_j |a_ij| max(|lo_j|, |hi_j|), so each side is moved out by
-// 4 eps S_i + the smallest normal number (for underflow): the box contains the exact image of the root box.  An empty
-// box (min = +inf, max = -inf) and a zero centre for a matrix without an inverse.
-template <typename T>
-BVH_HD void prepare_instance(Instance<T>& rec, typename ViewTypes<T>::BBox& box, typename ViewTypes<T>::Vec& centre) {
+// The inverse of the 3 x 4 affine map m (both builds) into inv: the adjugate of A over its determinant, then
+// -(A^-1 b); all NaN, and false, when an entry of m is not finite, the determinant is 0 or not finite, or an entry of
+// the inverse is not finite.  prepare_instance's world_to_object, and the placement of a motion record at a time.
+template <typename T> BVH_HD bool invert_affine(const T* m, T* out) {
     using R = bvhb200::Real<T>;
     using UI = typename R::UInt;
-    const T inf = R::from_bits(sizeof(T) == 4 ? (UI)0x7F800000u : (UI)0x7FF0000000000000ull);
     const T nan = R::from_bits(~(UI)0 >> 1);
-    const T* m = rec.object_to_world;
     bool ok = true;
     for (int k = 0; k < 12; ++k) ok = ok && R::is_finite(m[k]);
     const T a[3][3] = { { m[0], m[1], m[2] }, { m[4], m[5], m[6] }, { m[8], m[9], m[10] } };
@@ -671,25 +732,106 @@ BVH_HD void prepare_instance(Instance<T>& rec, typename ViewTypes<T>::BBox& box,
     const T b[3] = { m[3], m[7], m[11] };
     for (int i = 0; i < 3; ++i) inv[4 * i + 3] = R::neg(affine_row(inv + 4 * i, b, false));
     for (int k = 0; k < 12; ++k) ok = ok && R::is_finite(inv[k]);
-    for (int k = 0; k < 12; ++k) rec.world_to_object[k] = ok ? inv[k] : nan;
+    for (int k = 0; k < 12; ++k) out[k] = ok ? inv[k] : nan;
+    return ok;
+}
 
+// Axis i of the world box of the root box rb (minx, maxx, miny, maxy, minz, maxz) under the 3 x 4 map m (both builds):
+// b_i plus the sums of min / max(a_ij lo_j, a_ij hi_j), which in exact arithmetic is the box of the eight transformed
+// corners.  Its rounding error is below 2.5 eps S_i, S_i = |b_i| + sum_j |a_ij| max(|lo_j|, |hi_j|) (returned in s), so
+// each side is moved out by 4 eps S_i + the smallest normal number (for underflow): [lo, hi] contains the exact image of
+// the root box.  An overflow to NaN gives the whole axis on that side.
+template <typename T> BVH_HD void world_box_axis(const T* m, const T* rb, int i, T& lo, T& hi, T& s) {
+    using R = bvhb200::Real<T>;
+    using UI = typename R::UInt;
+    const T inf = R::from_bits(sizeof(T) == 4 ? (UI)0x7F800000u : (UI)0x7FF0000000000000ull);
+    const T pad = R::mul(R::eps(), T(4)), tiny = sizeof(T) == 4 ? (T)FLT_MIN : (T)DBL_MIN;
+    T l = m[4 * i + 3], h = m[4 * i + 3];
+    s = R::abs(m[4 * i + 3]);
+    for (int j = 0; j < 3; ++j) {
+        const T p = R::mul(m[4 * i + j], rb[2 * j]), q = R::mul(m[4 * i + j], rb[2 * j + 1]);
+        l = R::add(l, p < q ? p : q);
+        h = R::add(h, p < q ? q : p);
+        const T e = R::abs(rb[2 * j]) < R::abs(rb[2 * j + 1]) ? R::abs(rb[2 * j + 1]) : R::abs(rb[2 * j]);
+        s = R::add(s, R::mul(R::abs(m[4 * i + j]), e));
+    }
+    const T d = R::add(R::mul(s, pad), tiny);
+    lo = R::sub(l, d);
+    hi = R::add(h, d);
+    if (lo != lo) lo = R::neg(inf);     // (an overflow: the whole axis)
+    if (hi != hi) hi = inf;
+}
+
+// prepare_instances for one record (both builds).  root_index: the bottom root's.  world_to_object: invert_affine of
+// object_to_world.  The box: world_box_axis of the bottom root box, which contains the exact image of the root box; an
+// empty box (min = +inf, max = -inf) and a zero centre for a matrix without an inverse.
+template <typename T>
+BVH_HD void prepare_instance(Instance<T>& rec, typename ViewTypes<T>::BBox& box, typename ViewTypes<T>::Vec& centre) {
+    using R = bvhb200::Real<T>;
+    using UI = typename R::UInt;
+    const T inf = R::from_bits(sizeof(T) == 4 ? (UI)0x7F800000u : (UI)0x7FF0000000000000ull);
+    const T* m = rec.object_to_world;
+    const bool ok = invert_affine(m, rec.world_to_object);
     rec.root_index = rec.nodes[1].index;
     const T* rb = rec.nodes[1].bounds;  // the bottom root box: minx, maxx, miny, maxy, minz, maxz
-    const T pad = R::mul(R::eps(), T(4)), tiny = sizeof(T) == 4 ? (T)FLT_MIN : (T)DBL_MIN;
     T lo[3], hi[3], mid[3];
     for (int i = 0; i < 3; ++i) {
-        T l = m[4 * i + 3], h = m[4 * i + 3], s = R::abs(m[4 * i + 3]);
-        for (int j = 0; j < 3; ++j) {
-            const T p = R::mul(m[4 * i + j], rb[2 * j]), q = R::mul(m[4 * i + j], rb[2 * j + 1]);
-            l = R::add(l, p < q ? p : q);
-            h = R::add(h, p < q ? q : p);
-            const T e = R::abs(rb[2 * j]) < R::abs(rb[2 * j + 1]) ? R::abs(rb[2 * j + 1]) : R::abs(rb[2 * j]);
-            s = R::add(s, R::mul(R::abs(m[4 * i + j]), e));
-        }
-        const T d = R::add(R::mul(s, pad), tiny);
-        lo[i] = R::sub(l, d);
-        hi[i] = R::add(h, d);
-        if (lo[i] != lo[i]) lo[i] = R::neg(inf);              // (an overflow: the whole axis)
+        T s;
+        world_box_axis(m, rb, i, lo[i], hi[i], s);
+        mid[i] = R::mul(R::add(lo[i], hi[i]), T(0.5));
+        if (!R::is_finite(mid[i])) mid[i] = T(0);
+        if (!ok) { lo[i] = inf; hi[i] = R::neg(inf); mid[i] = T(0); }
+    }
+    box.min.x = lo[0]; box.min.y = lo[1]; box.min.z = lo[2];
+    box.max.x = hi[0]; box.max.y = hi[1]; box.max.z = hi[2];
+    centre.x = mid[0]; centre.y = mid[1]; centre.z = mid[2];
+}
+
+// The placement of a motion record at `time` (both builds; instance_at is its public form).  tau is time clamped to
+// [0, 1], a NaN time counting as 0.  Each coefficient is key0[k] at tau == 0, key1[k] at tau == 1, key0[k] where the
+// keys agree, and otherwise (1 - tau) key0[k] + tau key1[k] rounded step by step (sub, mul, mul, add; never an FMA).
+// The endpoints and every coefficient that does not move are exact.
+template <typename T> BVH_HD void blend_keys(const T (&keys)[2][12], T time, T* m) {
+    using R = bvhb200::Real<T>;
+    const T tau = time > T(0) ? (time < T(1) ? time : T(1)) : T(0);       // (a NaN fails both tests: 0)
+    const T rest = R::sub(T(1), tau);
+    for (int k = 0; k < 12; ++k) {
+        const T k0 = keys[0][k], k1 = keys[1][k];
+        m[k] = tau == T(0) ? k0 : tau == T(1) ? k1 : k0 == k1 ? k0 : R::add(R::mul(rest, k0), R::mul(tau, k1));
+    }
+}
+
+// prepare_motion_instances for one record (both builds).  root_index: the bottom root's.  The box holds the bottom
+// root box at every time of the shutter, under the placement blend_keys computes:
+//   * in exact arithmetic, the image of a point p under (1 - tau) M0 + tau M1 is the convex combination
+//     (1 - tau) M0 p + tau M1 p of its images under the keys, so it lies in the union of world_box_axis' box at each
+//     key (each contains the exact image of the root box, whether or not the key has an inverse);
+//   * blend_keys rounds each moving coefficient three times (1 - tau, the two products, the sum: the first is exact
+//     for tau >= 1/2), so it is within 1.5 eps max(|k0|, |k1|) (1 + O(eps)) of the exact blend, and the image of a
+//     root-box point moves by at most 1.5 eps (S0_i + S1_i) (1 + O(eps)), with S0_i, S1_i world_box_axis' S_i at
+//     the keys;
+//   * so each side of the union is moved out by a further 3 eps (S0_i + S1_i) + the smallest normal number: the
+//     margin beyond 1.5 eps covers the rounding of that widening (at most eps/2 of a bound below S0_i + S1_i).
+// A key with a non-finite entry gives the empty box and a zero centre: no ray reaches the record.
+template <typename T>
+BVH_HD void prepare_motion_instance(MotionInstance<T>& rec, typename ViewTypes<T>::BBox& box, typename ViewTypes<T>::Vec& centre) {
+    using R = bvhb200::Real<T>;
+    using UI = typename R::UInt;
+    const T inf = R::from_bits(sizeof(T) == 4 ? (UI)0x7F800000u : (UI)0x7FF0000000000000ull);
+    const T pad = R::mul(R::eps(), T(3)), tiny = sizeof(T) == 4 ? (T)FLT_MIN : (T)DBL_MIN;
+    bool ok = true;
+    for (int k = 0; k < 12; ++k) ok = ok && R::is_finite(rec.object_to_world[0][k]) && R::is_finite(rec.object_to_world[1][k]);
+    rec.root_index = rec.nodes[1].index;
+    const T* rb = rec.nodes[1].bounds;
+    T lo[3], hi[3], mid[3];
+    for (int i = 0; i < 3; ++i) {
+        T lo0, hi0, s0, lo1, hi1, s1;
+        world_box_axis(rec.object_to_world[0], rb, i, lo0, hi0, s0);
+        world_box_axis(rec.object_to_world[1], rb, i, lo1, hi1, s1);
+        const T d = R::add(R::mul(R::add(s0, s1), pad), tiny);
+        lo[i] = R::sub(lo1 < lo0 ? lo1 : lo0, d);
+        hi[i] = R::add(hi0 < hi1 ? hi1 : hi0, d);
+        if (lo[i] != lo[i]) lo[i] = R::neg(inf);
         if (hi[i] != hi[i]) hi[i] = inf;
         mid[i] = R::mul(R::add(lo[i], hi[i]), T(0.5));
         if (!R::is_finite(mid[i])) mid[i] = T(0);
@@ -717,6 +859,56 @@ BVH_HD void instance_leaf(const Shader& shader, const bvhb200::DevTri<T>* tris, 
         return true;
     });
 }
+
+template <typename T, typename Shader> struct MotionShader {
+    using Ray = typename ViewTypes<T>::Ray;
+    using Hit = typename ViewTypes<T>::Hit;
+    struct Payload {
+        typename Shader::Payload user;
+        T time;                         // the ray's (path's) time, as start gave it
+    };
+    Shader shader;
+    // trace_instances
+    BVH_HD Ray start(size_t i, Payload& p) const { return shader.start(i, p.user, p.time); }
+    BVH_HD void finish(size_t i, const Payload& p, const Hit& hit, uint32_t inst) const { shader.finish(i, p.user, hit, inst); }
+    // trace_instance_paths
+    BVH_HD PathStep start(size_t i, Payload& p, Ray& ray) const { return shader.start(i, p.user, ray, p.time); }
+    BVH_HD PathStep next(size_t i, Payload& p, const Hit& hit, uint32_t inst, Ray& ray) const {
+        return shader.next(i, p.user, hit, inst, ray);
+    }
+    BVH_HD void finish(size_t i, const Payload& p) const { shader.finish(i, p.user); }
+    // both
+    BVH_HD bool accept(Payload& p, uint32_t inst, size_t prim_id, T t, T u, T v) const {
+        return static_cast<bool>(shader.accept(p.user, inst, prim_id, t, u, v));
+    }
+};
+
+// The placement a ray meets a record at, as its world_to_object handed to f (both builds): a static record's own; for
+// a motion record, the inverse of blend_keys at the payload's time (instance_at's), built here.  All NaN: no inverse.
+template <typename T, typename Payload, typename F>
+BVH_HD void with_world_to_object(const Instance<T>& rec, const Payload&, F&& f) { f(static_cast<const T*>(rec.world_to_object)); }
+template <typename T, typename Payload, typename F>
+BVH_HD void with_world_to_object(const MotionInstance<T>& rec, const Payload& payload, F&& f) {
+    T m[12], inv[12];
+    blend_keys(rec.object_to_world, payload.time, m);
+    invert_affine(m, inv);
+    f(static_cast<const T*>(inv));
+}
+}
+
+// The placement of motion record `rec` at `time` (both builds): the Instance<T> the motion forms of trace_instances and
+// trace_instance_paths trace a ray of that time through.  Its object_to_world is the blend of the keys
+// (detail::blend_keys: time clamped to [0, 1], a NaN time as 0; exact at 0 and 1 and for coefficients that do not
+// move), its world_to_object prepare_instance's inverse of that (all NaN when it has none: the ray skips the record),
+// and root_index, depth and the bottom arrays are the record's.
+template <typename T> BVH_HD Instance<T> instance_at(const MotionInstance<T>& rec, T time) {
+    Instance<T> out;
+    out.nodes = rec.nodes; out.prim_ids = rec.prim_ids; out.tris = rec.tris;
+    out.root_index = rec.root_index;
+    out.depth = rec.depth;
+    detail::blend_keys(rec.object_to_world, time, out.object_to_world);
+    detail::invert_affine(out.object_to_world, out.world_to_object);
+    return out;
 }
 
 #if defined(__CUDACC__)
@@ -827,6 +1019,37 @@ __device__ __forceinline__ void enter_instance(const InstanceShader<T, Shader>& 
     inst = id;
     top = rec->root_index;
 }
+// enter_motion_instance: enter_instance for motion records: the placement at the time in the lane's payload is built
+// first (with_world_to_object), and the instance is skipped when it has no inverse at that time.  A separate function
+// rather than a form of enter_instance: every shared form tried changed the register assignment of
+// device_view_instance_kernel for static records (DESIGN.md section 8).
+template <typename T, bool IsRobust, typename U, typename Shader, typename Payload>
+__device__ __forceinline__ void enter_motion_instance(const InstanceShader<T, Shader>& is, const Payload& payload,
+                                                      bvhb200::SmemStack<U>& stack, bvhb200::RayCtx<T>& r, uint32_t& inst, U& top) {
+    using R = bvhb200::Real<T>;
+    const U first = bvhb200::index_first(top);
+    const uint32_t count = bvhb200::index_count(top);
+    const uint32_t id = is.prim_ids[first];
+    const MotionInstance<T>* rec = is.records + id;
+    const U rest = bvhb200::make_index<U>(first + 1, count - 1);
+    with_world_to_object(*rec, payload, [&](const T* world_to_object) {
+        if (instance_is_singular(world_to_object)) {
+            top = count > 1 ? rest : bvhb200::pop_or_done<U>(stack);
+            return;
+        }
+        if (count > 1) stack.push(rest);
+        for (int k = 0; k < 3; ++k) stack.push(R::bits(r.org[k]));
+        for (int k = 0; k < 3; ++k) stack.push(R::bits(r.dir[k]));
+        stack.push(kInstanceMarker<U>);
+        object_ray(world_to_object, r, r);
+        bvhb200::ray_prologue<T, IsRobust>(r);
+        inst = id;
+        top = rec->root_index;
+    });
+}
+// Whether a shader runs motion records
+template <typename Shader> struct IsMotion : std::false_type {};
+template <typename T, typename Shader> struct IsMotion<MotionShader<T, Shader>> : std::true_type {};
 // walk_levels: the level changes the entry in `top` asks for, until the lane holds a node of some tree (or
 // kTraversalDone: the top level's stack is empty): leave() (leave_instance) on the marker, enter() (enter_instance) on a
 // leaf of the top tree
@@ -1202,14 +1425,17 @@ device_view_instance_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsig
     // the marker was popped: the world ray back, with the current tmax, and the next entry of the top level
     auto leave = [&] { detail::leave_instance<T, IsRobust>(stack, r, inst, top); };
     // `top` is a leaf of the top tree: enter its first instance, or go past it when it is singular
-    auto enter = [&] { detail::enter_instance<T, IsRobust>(is, stack, r, inst, top); };
+    auto enter = [&] {
+        if constexpr (detail::IsMotion<Shader>::value) detail::enter_motion_instance<T, IsRobust>(is, payload, stack, r, inst, top);
+        else detail::enter_instance<T, IsRobust>(is, stack, r, inst, top);
+    };
 
     // leaf phase: a bottom leaf's triangles through the filter (the ray ends on an any-hit hit), then the level changes
     // the next entry asks for, until the lane holds a node of some tree; the ray ends when the top level's stack is empty
     auto leaf = [&] {
         if (!has_ray || bvhb200::index_count(top) == 0) return;
         if (inst != detail::kNoInstance && top != kMarker) {
-            const Instance<T>* rec = is.records + inst;
+            const auto* rec = is.records + inst;
             detail::instance_leaf<T, TieLastVisited>(is.shader, rec->tris, rec->prim_ids, inst, payload, (uint32_t)bvhb200::index_first(top),
                                                      bvhb200::index_count(top), r, hit, hit_inst);
             if (IsAnyHit && hit.slot != bvhb200::kInvalidId) { retire(); return; }
@@ -1313,14 +1539,17 @@ device_view_instance_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, 
     };
 
     auto leave = [&] { detail::leave_instance<T, IsRobust>(stack, r, inst, top); };
-    auto enter = [&] { detail::enter_instance<T, IsRobust>(is, stack, r, inst, top); };
+    auto enter = [&] {
+        if constexpr (detail::IsMotion<Shader>::value) detail::enter_motion_instance<T, IsRobust>(is, payload, stack, r, inst, top);
+        else detail::enter_instance<T, IsRobust>(is, stack, r, inst, top);
+    };
 
     // leaf phase: a bottom leaf's triangles through the filter, then the level walk of device_view_instance_kernel; the
     // segment ends on an occlusion hit or when the top level is done (kTraversalDone, also a NaN segment's start)
     auto leaf = [&] {
         if (!has_path || bvhb200::index_count(top) == 0) return;
         if (inst != detail::kNoInstance && top != kMarker) {
-            const Instance<T>* rec = is.records + inst;
+            const auto* rec = is.records + inst;
             detail::instance_leaf<T, TieLastVisited>(is.shader, rec->tris, rec->prim_ids, inst, payload, (uint32_t)bvhb200::index_first(top),
                                                      bvhb200::index_count(top), r, hit, hit_inst);
             if (occlusion && hit.slot != bvhb200::kInvalidId) { end_segment(); return; }
@@ -1339,6 +1568,14 @@ __global__ void prepare_instances_kernel(Instance<T>* records, size_t count, typ
                                          typename detail::ViewTypes<T>::Vec* centers) {
     const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i < count) detail::prepare_instance<T>(records[i], bboxes[i], centers[i]);
+}
+
+// The kernel of prepare_motion_instances: one thread per motion record.
+template <typename T>
+__global__ void prepare_motion_instances_kernel(MotionInstance<T>* records, size_t count, typename detail::ViewTypes<T>::BBox* bboxes,
+                                                typename detail::ViewTypes<T>::Vec* centers) {
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i < count) detail::prepare_motion_instance<T>(records[i], bboxes[i], centers[i]);
 }
 #endif
 
@@ -1616,27 +1853,24 @@ template <typename T> struct DeviceView {
     template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
     void trace_instances(size_t n, const Instances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes,
                          void* on_stream) const {
-        if (instances.count != prim_count || (instances.count && !instances.records))
-            throw std::invalid_argument("bvh::v2::cuda::DeviceView::trace_instances: " + std::to_string(instances.count) +
-                                        " instance records for a top tree of " + std::to_string(prim_count) + " primitives");
-        const bvhb200::TracePlan plan = batch_plan<IsAnyHit, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
-        const detail::InstanceShader<T, Shader> is { shader, instances.records, prim_ids };
-        const size_t extra = instances.max_depth + detail::kInstanceStackExtra;
-#if defined(__CUDACC__)
-        run_batch("trace_instances", device_view_instance_kernel<T, IsAnyHit, IsRobust, TieLastVisited, Shader>, is, n, plan.refill_min,
-                  plan.inner_budget, workspace, workspace_bytes, on_stream, extra);
-#else
-        (void)on_stream; (void)plan;
-        batch_stack_bytes("trace_instances", workspace, workspace_bytes, extra);
-        using Payload = typename Shader::Payload;
-        for (size_t i = 0; i < n; ++i) {
-            Payload payload;
-            const Ray ray = shader.start(i, payload);
-            uint32_t hit_inst = detail::kNoInstance;
-            const Hit hit = host_instance_ray<IsAnyHit, IsRobust, TieLastVisited>(is, payload, ray, hit_inst);
-            shader.finish(i, static_cast<const Payload&>(payload), hit, hit_inst);
-        }
-#endif
+        instance_batch<IsAnyHit, IsRobust, TieLastVisited>("trace_instances", n, instances,
+                                                           detail::InstanceShader<T, Shader> { shader, instances.records, prim_ids },
+                                                           workspace, workspace_bytes, on_stream);
+    }
+    // The same through a top-level tree of moving placements, each ray at its own time: see "Motion blur" at the top of
+    // this file.  The shader's start also gives the ray's time.
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instances(size_t n, const MotionInstances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes) const {
+        trace_instances<IsAnyHit, IsRobust, TieLastVisited>(n, instances, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instances(size_t n, const MotionInstances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes,
+                         void* on_stream) const {
+        using MS = detail::MotionShader<T, Shader>;
+        instance_batch<IsAnyHit, IsRobust, TieLastVisited>("trace_instances (motion)", n, instances,
+                                                           detail::InstanceShader<T, MS> { MS { shader }, instances.records, prim_ids },
+                                                           workspace, workspace_bytes, on_stream);
     }
 
     // Whole paths through a top-level tree of placed meshes, each segment continued in place from the last: see "Paths
@@ -1650,32 +1884,25 @@ template <typename T> struct DeviceView {
     template <bool IsRobust, bool TieLastVisited = false, typename Shader>
     void trace_instance_paths(size_t n, const Instances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes,
                               void* on_stream) const {
-        if (instances.count != prim_count || (instances.count && !instances.records))
-            throw std::invalid_argument("bvh::v2::cuda::DeviceView::trace_instance_paths: " + std::to_string(instances.count) +
-                                        " instance records for a top tree of " + std::to_string(prim_count) + " primitives");
-        const bvhb200::TracePlan plan = batch_plan<false, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
-        const detail::InstanceShader<T, Shader> is { shader, instances.records, prim_ids };
-        const size_t extra = instances.max_depth + detail::kInstanceStackExtra;
-#if defined(__CUDACC__)
-        run_batch("trace_instance_paths", device_view_instance_path_kernel<T, IsRobust, TieLastVisited, Shader>, is, n, plan.refill_min,
-                  plan.inner_budget, workspace, workspace_bytes, on_stream, extra);
-#else
-        (void)on_stream; (void)plan;
-        batch_stack_bytes("trace_instance_paths", workspace, workspace_bytes, extra);
-        using Payload = typename Shader::Payload;
-        for (size_t i = 0; i < n; ++i) {
-            Payload payload;
-            Ray ray;
-            PathStep step = shader.start(i, payload, ray);
-            while (step != PathStep::End) {
-                uint32_t hit_inst = detail::kNoInstance;
-                const Hit hit = step == PathStep::Occlusion ? host_instance_ray<true, IsRobust, TieLastVisited>(is, payload, ray, hit_inst)
-                                                            : host_instance_ray<false, IsRobust, TieLastVisited>(is, payload, ray, hit_inst);
-                step = shader.next(i, payload, hit, hit_inst, ray);
-            }
-            shader.finish(i, static_cast<const Payload&>(payload));
-        }
-#endif
+        instance_path_batch<IsRobust, TieLastVisited>("trace_instance_paths", n, instances,
+                                                      detail::InstanceShader<T, Shader> { shader, instances.records, prim_ids },
+                                                      workspace, workspace_bytes, on_stream);
+    }
+    // The same through a top-level tree of moving placements, each path at its own time: see "Motion blur" at the top of
+    // this file.  The shader's start also gives the path's time, which holds for all its segments.
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instance_paths(size_t n, const MotionInstances<T>& instances, const Shader& shader, void* workspace,
+                              size_t workspace_bytes) const {
+        trace_instance_paths<IsRobust, TieLastVisited>(n, instances, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instance_paths(size_t n, const MotionInstances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes,
+                              void* on_stream) const {
+        using MS = detail::MotionShader<T, Shader>;
+        instance_path_batch<IsRobust, TieLastVisited>("trace_instance_paths (motion)", n, instances,
+                                                      detail::InstanceShader<T, MS> { MS { shader }, instances.records, prim_ids },
+                                                      workspace, workspace_bytes, on_stream);
     }
 
     // PrecomputedTri::intersect (reference tri.h:55-74) on BVH-order triangle k: true, with the hit's distance and
@@ -1704,6 +1931,67 @@ private:
         request.is_float = sizeof(T) == 4;
         request.n = n;
         return bvhb200::plan_trace(request);
+    }
+
+    // trace_instances of either record kind (Records: Instances<T> or MotionInstances<T>; `is` holds its records and the
+    // shader, wrapped in detail::MotionShader for motion records), named `call` in its errors.
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited, typename Records, typename Shader>
+    void instance_batch(const char* call, size_t n, const Records& instances, const detail::InstanceShader<T, Shader>& is, void* workspace,
+                        size_t workspace_bytes, void* on_stream) const {
+        check_instances(call, instances.count, instances.records);
+        const bvhb200::TracePlan plan = batch_plan<IsAnyHit, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
+        const size_t extra = instances.max_depth + detail::kInstanceStackExtra;
+#if defined(__CUDACC__)
+        run_batch(call, device_view_instance_kernel<T, IsAnyHit, IsRobust, TieLastVisited, Shader>, is, n, plan.refill_min,
+                  plan.inner_budget, workspace, workspace_bytes, on_stream, extra);
+#else
+        (void)on_stream; (void)plan;
+        batch_stack_bytes(call, workspace, workspace_bytes, extra);
+        using Payload = typename Shader::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            const Ray ray = is.shader.start(i, payload);
+            uint32_t hit_inst = detail::kNoInstance;
+            const Hit hit = host_instance_ray<IsAnyHit, IsRobust, TieLastVisited>(is, payload, ray, hit_inst);
+            is.shader.finish(i, static_cast<const Payload&>(payload), hit, hit_inst);
+        }
+#endif
+    }
+
+    // trace_instance_paths of either record kind, as instance_batch
+    template <bool IsRobust, bool TieLastVisited, typename Records, typename Shader>
+    void instance_path_batch(const char* call, size_t n, const Records& instances, const detail::InstanceShader<T, Shader>& is,
+                             void* workspace, size_t workspace_bytes, void* on_stream) const {
+        check_instances(call, instances.count, instances.records);
+        const bvhb200::TracePlan plan = batch_plan<false, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
+        const size_t extra = instances.max_depth + detail::kInstanceStackExtra;
+#if defined(__CUDACC__)
+        run_batch(call, device_view_instance_path_kernel<T, IsRobust, TieLastVisited, Shader>, is, n, plan.refill_min,
+                  plan.inner_budget, workspace, workspace_bytes, on_stream, extra);
+#else
+        (void)on_stream; (void)plan;
+        batch_stack_bytes(call, workspace, workspace_bytes, extra);
+        using Payload = typename Shader::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            Ray ray;
+            PathStep step = is.shader.start(i, payload, ray);
+            while (step != PathStep::End) {
+                uint32_t hit_inst = detail::kNoInstance;
+                const Hit hit = step == PathStep::Occlusion ? host_instance_ray<true, IsRobust, TieLastVisited>(is, payload, ray, hit_inst)
+                                                            : host_instance_ray<false, IsRobust, TieLastVisited>(is, payload, ray, hit_inst);
+                step = is.shader.next(i, payload, hit, hit_inst, ray);
+            }
+            is.shader.finish(i, static_cast<const Payload&>(payload));
+        }
+#endif
+    }
+
+    // The record count of trace_instances and trace_instance_paths: the top tree's primitive count
+    void check_instances(const char* call, size_t count, const void* records) const {
+        if (count != prim_count || (count && !records))
+            throw std::invalid_argument(std::string("bvh::v2::cuda::DeviceView::") + call + ": " + std::to_string(count) +
+                                        " instance records for a top tree of " + std::to_string(prim_count) + " primitives");
     }
 
     // One ray of trace_triangles, and one segment of trace_paths, on the host: the library's traversal with the shader's
@@ -1750,10 +2038,14 @@ private:
                 [&](Index begin, Index end) {
                     for (Index k = begin; k < end; ++k) {
                         const uint32_t id = prim_ids[k];
-                        const Instance<T>& rec = is.records[id];
-                        if (detail::instance_is_singular(rec.world_to_object)) continue;
+                        const auto& rec = is.records[id];
+                        bool singular = false;
                         bvhb200::RayCtx<T> o;
-                        detail::object_ray(rec.world_to_object, r, o);
+                        detail::with_world_to_object(rec, payload, [&](const T* world_to_object) {
+                            singular = detail::instance_is_singular(world_to_object);
+                            detail::object_ray(world_to_object, r, o);
+                        });
+                        if (singular) continue;
                         bvhb200::ray_prologue<T, IsRobust>(o);
                         detail::VectorStack<Index> bottom;
                         bottom.elems.reserve(rec.depth + 1);
@@ -1880,6 +2172,46 @@ void prepare_instances(const Instances<T>& instances, typename detail::ViewTypes
 #else
     (void)stream;
     for (size_t i = 0; i < instances.count; ++i) detail::prepare_instance<T>(instances.records[i], bboxes[i], centers[i]);
+#endif
+}
+
+// A motion record of the mesh `view` (which must have triangles) placed by `key0` at time 0 and `key1` at time 1 (12
+// values each, 3 x 4 row-major), on the host or the device.  root_index is 0 until prepare_motion_instances writes it.
+template <typename T> BVH_HD MotionInstance<T> make_motion_instance(const DeviceView<T>& view, const T* key0, const T* key1) {
+    MotionInstance<T> rec;
+    rec.nodes = view.nodes; rec.prim_ids = view.prim_ids; rec.tris = view.tris;
+    rec.root_index = 0;
+    rec.depth = static_cast<uint32_t>(view.depth);
+    for (int k = 0; k < 12; ++k) {
+        rec.object_to_world[0][k] = key0[k];
+        rec.object_to_world[1][k] = key1[k];
+    }
+    return rec;
+}
+
+// prepare_instances for motion records (one thread each, stream-ordered on `stream`, no host synchronisation): every
+// root index, and in bboxes[i] / centers[i] a world box that holds record i's bottom root box at every time of the
+// shutter, and its centre, ready for bvhNN_build_boxes or bvhNN_refit_boxes with BVH_DEVICE_POINTERS.  See
+// detail::prepare_motion_instance for the bound.  A key with a non-finite entry gives an empty box; a key without an
+// inverse does not (the rays at times where the placement has none skip the record).  The current device must be the
+// records'.  A failed launch throws std::runtime_error.  Compiled as plain host C++, the records are prepared serially
+// in place.
+template <typename T>
+void prepare_motion_instances(const MotionInstances<T>& instances, typename detail::ViewTypes<T>::BBox* bboxes,
+                              typename detail::ViewTypes<T>::Vec* centers, void* stream = nullptr) {
+    if (instances.count == 0) return;
+    if (!instances.records || !bboxes || !centers)
+        throw std::invalid_argument("bvh::v2::cuda::prepare_motion_instances: null records, boxes or centres");
+#if defined(__CUDACC__)
+    const unsigned block = 128, grid = (unsigned)((instances.count + block - 1) / block);
+    prepare_motion_instances_kernel<T><<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(instances.records, instances.count, bboxes,
+                                                                                           centers);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess)
+        throw std::runtime_error(std::string("bvh::v2::cuda::prepare_motion_instances: launch: ") + cudaGetErrorString(e));
+#else
+    (void)stream;
+    for (size_t i = 0; i < instances.count; ++i) detail::prepare_motion_instance<T>(instances.records[i], bboxes[i], centers[i]);
 #endif
 }
 
