@@ -82,6 +82,8 @@ INSTANCE_PATH_TRACE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_instance_p
 INSTANCE_PATH_TRACE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_instance_path_trace_kernels.so")
 MOTION_INSTANCE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_motion_instance_kernels.cu")
 MOTION_INSTANCE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_motion_instance_kernels.so")
+MOTION_TRIANGLE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_motion_triangle_kernels.cu")
+MOTION_TRIANGLE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_motion_triangle_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -172,6 +174,14 @@ def build_device_motion_instance_tests(force: bool = False, verbose: bool = Fals
     rays nested by hand one thread each, a path tracer with a time per path as one call and as a wavefront loop, the
     benchmark's plain shader)."""
     return _build_test_kernels(MOTION_INSTANCE_KERNELS_SRC, MOTION_INSTANCE_KERNELS_LIB, force, verbose)
+
+
+def build_device_motion_triangle_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_motion_triangle_kernels.cu: the test shaders of the motion forms of DeviceView::trace_triangles and
+    trace_paths, prepare_motion_triangles and triangle_at (a recording shader with a time per ray, the same rays nested
+    by hand one thread each, a path tracer with a time per path as one call, as a wavefront loop and as the static call,
+    the benchmark's plain shader and traversal counts)."""
+    return _build_test_kernels(MOTION_TRIANGLE_KERNELS_SRC, MOTION_TRIANGLE_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

@@ -516,6 +516,48 @@
 //     bvh3f_refit_boxes(top_bvh, d_boxes, count, BVH_DEVICE_POINTERS);    // on the top handle's stream
 //     top.trace_instances<false, false>(n, instances, Shade { d_rays, d_times, d_hits, d_inst }, workspace, bytes, stream);
 //
+// Deforming meshes: vertices that move over the shutter (skinning, cloth, a fluid surface).  MotionTriangles<T>
+// { vertices[2], count } views two vertex keys in device memory, vertices[0] at time 0 and vertices[1] at time 1, each
+// count x 9 values (p0 p1 p2) in original primitive order, the layout bvhNN_build_triangles, bvhNN_set_triangles and
+// bvhNN_refit_triangles take; the same pointer twice is a static mesh.  A ray at time tau sees triangle id as
+// triangle_at(tris, id, tau, v): each coordinate blended as a motion record's coefficients are (detail::blend_key: tau
+// clamped to [0, 1], a NaN time as 0; the key at 0 and 1 and where the keys agree, else (1 - tau) k0 + tau k1 by sub,
+// mul, mul, add, never an FMA).  prepare_motion_triangles(tris, bboxes, centers[, stream]) writes, per original id, a box
+// that holds triangle_at at every time of the shutter (the union of the key boxes, widened per moving axis for the
+// rounding of the blend; exactly tri_bounds_center's box when the keys are equal) and the centre of the triangle at 0.5,
+// for bvhNN_build_boxes / bvhNN_refit_boxes, in one stream-ordered kernel.  A key with a non-finite entry gives the empty
+// box.  On a view of a tree over those boxes (it needs no attached triangles):
+//     view.trace_triangles<IsAnyHit, IsRobust, TieLastVisited = false>(n, motion_tris, shader, workspace, bytes[, stream]);
+//     view.trace_paths<IsRobust, TieLastVisited = false>(n, motion_tris, shader, workspace, bytes[, stream]);
+// take the shaders of the static calls, except that start also gives the ray's (path's) time:
+//     Ray      start(size_t i, Payload& p, T& time) const;                     // trace_triangles
+//     PathStep start(size_t i, Payload& p, Ray& ray, T& time) const;           // trace_paths: for every segment
+//   * per ray (segment), the calls are exactly those of the static call on the same tree with its triangles replaced by
+//     precompute_tri(triangle_at(motion_tris, id, time)): the same accept calls (original id, bits of t, u, v) in the
+//     same order, the same record and, for paths, the same next calls.  With equal keys the motion call is the static
+//     call bit for bit at any time;
+//   * errors, checked on the host before any launch: motion_tris.count other than the tree's prim_count, or a null key
+//     pointer, throws std::invalid_argument; a small workspace or a stack beyond 200 KB std::length_error; a failed launch
+//     std::runtime_error; the messages name "trace_triangles (motion)" or "trace_paths (motion)".  Streams, the
+//     workspace, n == 0, the warp subset and the host build are those of the static calls;
+//   * the kernels are the static ones (device_view_triangle_kernel, device_view_path_kernel) under detail::MotionShader,
+//     which keeps the time beside the payload; the leaf loads each slot's original id and both keys (72 bytes in float),
+//     blends them and runs the library's tri_test on precompute_tri of the result, one triangle at a time.
+// One frame of a renderer (INTEGRATION.md §5 has it whole):
+//
+//     struct Shade {
+//         struct Payload {};
+//         const bvh_ray3f* rays; const float* times; bvh_hit3f* hits;
+//         __device__ bvh_ray3f start(size_t i, Payload&, float& time) const { time = times[i]; return rays[i]; }
+//         __device__ bool accept(Payload&, size_t, float, float, float) const { return true; }
+//         __device__ void finish(size_t i, const Payload&, const bvh_hit3f& h) const { hits[i] = h; }
+//     };
+//     skin<<<...>>>(d_key0, d_key1);                                  // yours: the vertices at the shutter's open and close
+//     const MotionTriangles<float> mesh { { d_key0, d_key1 }, count };
+//     prepare_motion_triangles(mesh, d_boxes, d_centres, stream);
+//     bvh3f_refit_boxes(bvh, d_boxes, count, BVH_DEVICE_POINTERS);   // on the handle's stream (first frame: build_boxes)
+//     view.trace_triangles<false, false>(n, mesh, Shade { d_rays, d_times, d_hits }, workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -588,6 +630,17 @@ template <typename T> struct MotionInstances {
     size_t max_depth = 0;
 };
 
+// A triangle mesh whose vertices move over the shutter, for the motion forms of trace_triangles and trace_paths: the
+// vertices at time 0 (vertices[0]) and at time 1 (vertices[1]), each count x 9 values (p0, p1, p2 of each triangle) in
+// original primitive order, as bvhNN_build_triangles, bvhNN_set_triangles and bvhNN_refit_triangles take them, in
+// device memory of the caller's.  A ray at time tau sees triangle id as triangle_at(tris, id, tau).  The same pointer
+// twice is a static mesh.  The keys are read on the device through the read-only (non-coherent) cache: write them in an
+// earlier kernel or copy on the stream, never in the kernel that traces or reads them.
+template <typename T> struct MotionTriangles {
+    const T* vertices[2] = { nullptr, nullptr };
+    size_t count = 0;
+};
+
 namespace detail {
 template <typename T> struct ViewTypes;
 template <> struct ViewTypes<float>  {
@@ -643,10 +696,17 @@ template <typename T> BVH_HD typename ViewTypes<T>::Hit make_hit(const bvhb200::
     hit.prim_id = rec.prim_id; hit.t = rec.t; hit.u = rec.u; hit.v = rec.v;
     return hit;
 }
-// What the kernel of DeviceView::trace_triangles reads besides the nodes: the caller's shader and the tree's triangles.
+// The shader the motion forms of trace_triangles, trace_paths, trace_instances and trace_instance_paths run: the
+// caller's, with the ray's time kept beside its payload (so in the lane's registers) from start on; defined below.
+template <typename T, typename Shader> struct MotionShader;
+// The triangle source of a shader: the tree's BVH-order triangles, or the keys of MotionTriangles<T> under a MotionShader.
+template <typename T, typename Shader> struct TrianglesOf { using type = const bvhb200::DevTri<T>*; };
+template <typename T, typename Shader> struct TrianglesOf<T, MotionShader<T, Shader>> { using type = MotionTriangles<T>; };
+
+// What the kernel of DeviceView::trace_triangles reads besides the nodes: the caller's shader and the triangles.
 template <typename T, typename Shader> struct TriangleShader {
     Shader shader;
-    const bvhb200::DevTri<T>* tris;     // BVH order
+    typename TrianglesOf<T, Shader>::type tris;     // BVH order; for motion, the keys in original order
     const uint32_t* prim_ids;
 };
 // The triangle leaf of DeviceView::trace_triangles (both builds): the library's leaf_range over [first, first + count)
@@ -659,10 +719,6 @@ BVH_HD void shader_leaf(const TriangleShader<T, Shader>& ts, Payload& payload, u
                                return static_cast<bool>(ts.shader.accept(payload, static_cast<size_t>(ts.prim_ids[slot]), t, u, v));
                            });
 }
-
-// The shader the motion forms of trace_instances and trace_instance_paths run: the caller's, with the ray's time kept
-// beside its payload (so in the lane's registers) from start on; defined below.
-template <typename T, typename Shader> struct MotionShader;
 // The record kind of a shader: Instance<T>, or MotionInstance<T> under a MotionShader.
 template <typename T, typename Shader> struct RecordOf { using type = Instance<T>; };
 template <typename T, typename Shader> struct RecordOf<T, MotionShader<T, Shader>> { using type = MotionInstance<T>; };
@@ -787,18 +843,95 @@ BVH_HD void prepare_instance(Instance<T>& rec, typename ViewTypes<T>::BBox& box,
     centre.x = mid[0]; centre.y = mid[1]; centre.z = mid[2];
 }
 
-// The placement of a motion record at `time` (both builds; instance_at is its public form).  tau is time clamped to
-// [0, 1], a NaN time counting as 0.  Each coefficient is key0[k] at tau == 0, key1[k] at tau == 1, key0[k] where the
-// keys agree, and otherwise (1 - tau) key0[k] + tau key1[k] rounded step by step (sub, mul, mul, add; never an FMA).
-// The endpoints and every coefficient that does not move are exact.
+// The linear blend of two keys, the one rule of every motion form (blend_keys, triangle_at).  shutter_time is the time
+// clamped to [0, 1], a NaN time counting as 0; blend_key of one value, with tau = shutter_time(time) and rest = 1 - tau,
+// is k0 at tau == 0, k1 at tau == 1, k0 where the keys agree, and otherwise (1 - tau) k0 + tau k1 rounded step by step
+// (sub, mul, mul, add; never an FMA).  The endpoints and every value that does not move are exact.
+template <typename T> BVH_HD T shutter_time(T time) { return time > T(0) ? (time < T(1) ? time : T(1)) : T(0); }  // (NaN: 0)
+template <typename T> BVH_HD T blend_key(T k0, T k1, T tau, T rest) {
+    using R = bvhb200::Real<T>;
+    return tau == T(0) ? k0 : tau == T(1) ? k1 : k0 == k1 ? k0 : R::add(R::mul(rest, k0), R::mul(tau, k1));
+}
+// The placement of a motion record at `time` (both builds; instance_at is its public form): blend_key of each coefficient.
 template <typename T> BVH_HD void blend_keys(const T (&keys)[2][12], T time, T* m) {
     using R = bvhb200::Real<T>;
-    const T tau = time > T(0) ? (time < T(1) ? time : T(1)) : T(0);       // (a NaN fails both tests: 0)
+    const T tau = shutter_time(time);
     const T rest = R::sub(T(1), tau);
-    for (int k = 0; k < 12; ++k) {
-        const T k0 = keys[0][k], k1 = keys[1][k];
-        m[k] = tau == T(0) ? k0 : tau == T(1) ? k1 : k0 == k1 ? k0 : R::add(R::mul(rest, k0), R::mul(tau, k1));
+    for (int k = 0; k < 12; ++k) m[k] = blend_key(keys[0][k], keys[1][k], tau, rest);
+}
+// A key of a motion triangle, read once per use (on the device through the read-only cache)
+template <typename T> BVH_HD T load_key(const T* p) {
+#if defined(__CUDA_ARCH__)
+    return __ldg(p);
+#else
+    return *p;
+#endif
+}
+}
+
+// Triangle `id` of a deforming mesh at `time` (both builds), its three vertices p0, p1, p2 into v: each coordinate
+// blended from the two keys by the rule of the motion forms (detail::blend_key: time clamped to [0, 1], a NaN time as 0;
+// exact at 0 and 1 and for coordinates that do not move).  The motion forms of trace_triangles and trace_paths test a
+// ray of that time against precompute_tri of exactly these values; a shader may call it too (a normal at the ray's
+// time).  On the device it reads the keys through the read-only (non-coherent) cache (__ldg), so the keys must not be
+// written by the kernel that calls it: write them in an earlier kernel or copy on the stream.
+template <typename T> BVH_HD void triangle_at(const MotionTriangles<T>& tris, size_t id, T time, T v[9]) {
+    using R = bvhb200::Real<T>;
+    const T tau = detail::shutter_time(time);
+    const T rest = R::sub(T(1), tau);
+    const T* k0 = tris.vertices[0] + 9 * id;
+    const T* k1 = tris.vertices[1] + 9 * id;
+    for (int k = 0; k < 9; ++k) v[k] = detail::blend_key(detail::load_key(k0 + k), detail::load_key(k1 + k), tau, rest);
+}
+
+namespace detail {
+// prepare_motion_triangles for triangle `id` (both builds).  The box holds triangle_at(tris, id, tau) at every tau of
+// the shutter:
+//   * in exact arithmetic each coordinate (1 - tau) k0 + tau k1 lies between its two keys, so the triangle lies in the
+//     union of tri_bounds_center's boxes at the two keys;
+//   * blend_key rounds a moving coordinate three times (1 - tau, the two products, the sum: the first is exact for
+//     tau >= 1/2), so it is within 1.5 eps max(|k0|, |k1|) (1 + O(eps)) of the exact blend, and within 1.5 eps M_a
+//     (1 + O(eps)) on axis a, M_a = max(|lo_a|, |hi_a|) of the union;
+//   * so each side of an axis on which some coordinate moves is moved out by 3 eps M_a + the smallest normal number
+//     (for underflow): the rounding of that widening takes at most eps/2 (M_a + the widening) back.
+// An axis on which no coordinate moves is the keys' own (blend_key gives the shared value), so with equal keys the box
+// is tri_bounds_center's bit for bit.  The centre is tri_bounds_center's of triangle_at at 0.5 (with equal keys, the
+// static centre).  A key with a non-finite entry gives the empty box and a zero centre: no ray reaches the triangle.
+template <typename T>
+BVH_HD void prepare_motion_triangle(const MotionTriangles<T>& tris, size_t id, typename ViewTypes<T>::BBox& box,
+                                    typename ViewTypes<T>::Vec& centre) {
+    using R = bvhb200::Real<T>;
+    using UI = typename R::UInt;
+    const T inf = R::from_bits(sizeof(T) == 4 ? (UI)0x7F800000u : (UI)0x7FF0000000000000ull);
+    const T pad = R::mul(R::eps(), T(3)), tiny = sizeof(T) == 4 ? (T)FLT_MIN : (T)DBL_MIN;
+    T v0[9], v1[9], vm[9];
+    bool ok = true;
+    for (int k = 0; k < 9; ++k) {
+        v0[k] = load_key(tris.vertices[0] + 9 * id + k);
+        v1[k] = load_key(tris.vertices[1] + 9 * id + k);
+        ok = ok && R::is_finite(v0[k]) && R::is_finite(v1[k]);
     }
+    const T half = T(0.5), rest = R::sub(T(1), half);                     // triangle_at(tris, id, 0.5), from v0 and v1
+    for (int k = 0; k < 9; ++k) vm[k] = blend_key(v0[k], v1[k], half, rest);
+    T lo0[3], hi0[3], c0[3], lo1[3], hi1[3], c1[3], lom[3], him[3], lo[3], hi[3], mid[3];
+    bvhb200::tri_bounds_center(v0, lo0, hi0, c0);
+    bvhb200::tri_bounds_center(v1, lo1, hi1, c1);
+    bvhb200::tri_bounds_center(vm, lom, him, mid);
+    for (int a = 0; a < 3; ++a) {
+        lo[a] = lo1[a] < lo0[a] ? lo1[a] : lo0[a];
+        hi[a] = hi0[a] < hi1[a] ? hi1[a] : hi0[a];
+        const bool moves = v0[a] != v1[a] || v0[3 + a] != v1[3 + a] || v0[6 + a] != v1[6 + a];
+        if (moves) {
+            const T m = R::abs(lo[a]) < R::abs(hi[a]) ? R::abs(hi[a]) : R::abs(lo[a]);
+            const T d = R::add(R::mul(m, pad), tiny);
+            lo[a] = R::sub(lo[a], d);
+            hi[a] = R::add(hi[a], d);
+        }
+        if (!ok) { lo[a] = inf; hi[a] = R::neg(inf); mid[a] = T(0); }
+    }
+    box.min.x = lo[0]; box.min.y = lo[1]; box.min.z = lo[2];
+    box.max.x = hi[0]; box.max.y = hi[1]; box.max.z = hi[2];
+    centre.x = mid[0]; centre.y = mid[1]; centre.z = mid[2];
 }
 
 // prepare_motion_instances for one record (both builds).  root_index: the bottom root's.  The box holds the bottom
@@ -868,20 +1001,47 @@ template <typename T, typename Shader> struct MotionShader {
         T time;                         // the ray's (path's) time, as start gave it
     };
     Shader shader;
-    // trace_instances
+    // trace_triangles and trace_instances
     BVH_HD Ray start(size_t i, Payload& p) const { return shader.start(i, p.user, p.time); }
+    BVH_HD void finish(size_t i, const Payload& p, const Hit& hit) const { shader.finish(i, p.user, hit); }
     BVH_HD void finish(size_t i, const Payload& p, const Hit& hit, uint32_t inst) const { shader.finish(i, p.user, hit, inst); }
-    // trace_instance_paths
+    // trace_paths and trace_instance_paths
     BVH_HD PathStep start(size_t i, Payload& p, Ray& ray) const { return shader.start(i, p.user, ray, p.time); }
+    BVH_HD PathStep next(size_t i, Payload& p, const Hit& hit, Ray& ray) const { return shader.next(i, p.user, hit, ray); }
     BVH_HD PathStep next(size_t i, Payload& p, const Hit& hit, uint32_t inst, Ray& ray) const {
         return shader.next(i, p.user, hit, inst, ray);
     }
     BVH_HD void finish(size_t i, const Payload& p) const { shader.finish(i, p.user); }
-    // both
+    // the triangle calls, and the instance calls
+    BVH_HD bool accept(Payload& p, size_t prim_id, T t, T u, T v) const {
+        return static_cast<bool>(shader.accept(p.user, prim_id, t, u, v));
+    }
     BVH_HD bool accept(Payload& p, uint32_t inst, size_t prim_id, T t, T u, T v) const {
         return static_cast<bool>(shader.accept(p.user, inst, prim_id, t, u, v));
     }
 };
+
+// The triangle leaf of the motion forms of trace_triangles and trace_paths (both builds): shader_leaf with the triangles
+// built at the payload's time.  Per slot: the original id, both keys, the blend (triangle_at), precompute_tri and the
+// library's tri_test with the canonical tie rule on original ids (unless TieLastVisited) and the shader's accept as the
+// filter: the static leaf on precompute_tri(triangle_at(tris, id, time)).  Not unrolled, so one triangle's registers are
+// live at a time.
+template <typename T, bool TieLastVisited, typename Shader, typename Payload>
+BVH_HD void shader_leaf(const TriangleShader<T, MotionShader<T, Shader>>& ts, Payload& payload, uint32_t first, uint32_t count,
+                        bvhb200::RayCtx<T>& r, bvhb200::HitState<T>& hit) {
+#if defined(__CUDA_ARCH__)
+    #pragma unroll 1
+#endif
+    for (uint32_t slot = first; slot < first + count; ++slot) {
+        const uint32_t id = ts.prim_ids[slot];
+        T v[9];
+        triangle_at(ts.tris, id, payload.time, v);
+        const bvhb200::DevTri<T> tri = bvhb200::precompute_tri(v);
+        bvhb200::tri_test<T>(tri, slot, ts.prim_ids, !TieLastVisited, r, hit, [&](uint32_t, T t, T u, T w) {
+            return ts.shader.accept(payload, static_cast<size_t>(id), t, u, w);
+        });
+    }
+}
 
 // The placement a ray meets a record at, as its world_to_object handed to f (both builds): a static record's own; for
 // a motion record, the inverse of blend_keys at the payload's time (instance_at's), built here.  All NaN: no inverse.
@@ -1577,6 +1737,14 @@ __global__ void prepare_motion_instances_kernel(MotionInstance<T>* records, size
     const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i < count) detail::prepare_motion_instance<T>(records[i], bboxes[i], centers[i]);
 }
+
+// The kernel of prepare_motion_triangles: one thread per triangle.
+template <typename T>
+__global__ void prepare_motion_triangles_kernel(MotionTriangles<T> tris, typename detail::ViewTypes<T>::BBox* bboxes,
+                                                typename detail::ViewTypes<T>::Vec* centers) {
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i < tris.count) detail::prepare_motion_triangle<T>(tris, i, bboxes[i], centers[i]);
+}
 #endif
 
 // A plain-data view of one device tree (what bvhNN_get_device_view reports), passed to kernels by value.
@@ -1791,21 +1959,25 @@ template <typename T> struct DeviceView {
     void trace_triangles(size_t n, const Shader& shader, void* workspace, size_t workspace_bytes, void* on_stream) const {
         if (!tris)
             throw std::invalid_argument("bvh::v2::cuda::DeviceView::trace_triangles: the tree has no triangles (built from boxes)");
-        const bvhb200::TracePlan plan = batch_plan<IsAnyHit, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
-        const detail::TriangleShader<T, Shader> ts { shader, tris, prim_ids };
-#if defined(__CUDACC__)
-        run_batch("trace_triangles", device_view_triangle_kernel<T, IsAnyHit, IsRobust, TieLastVisited, Shader>, ts, n, plan.refill_min,
-                  plan.inner_budget, workspace, workspace_bytes, on_stream);
-#else
-        (void)on_stream; (void)plan;
-        batch_stack_bytes("trace_triangles", workspace, workspace_bytes);
-        using Payload = typename Shader::Payload;
-        for (size_t i = 0; i < n; ++i) {
-            Payload payload;
-            const Ray ray = shader.start(i, payload);
-            shader.finish(i, static_cast<const Payload&>(payload), host_triangle_ray<IsAnyHit, IsRobust, TieLastVisited>(ts, payload, ray));
-        }
-#endif
+        triangle_batch<IsAnyHit, IsRobust, TieLastVisited>("trace_triangles", n, detail::TriangleShader<T, Shader> { shader, tris, prim_ids },
+                                                           workspace, workspace_bytes, on_stream);
+    }
+    // The same through a mesh whose vertices move over the shutter, each ray at its own time: see "Deforming meshes" at
+    // the top of this file.  The view needs no triangles (a tree from bvhNN_build_boxes over prepare_motion_triangles'
+    // boxes is the usual one); the shader's start also gives the ray's time.
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_triangles(size_t n, const MotionTriangles<T>& motion, const Shader& shader, void* workspace, size_t workspace_bytes) const {
+        trace_triangles<IsAnyHit, IsRobust, TieLastVisited>(n, motion, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_triangles(size_t n, const MotionTriangles<T>& motion, const Shader& shader, void* workspace, size_t workspace_bytes,
+                         void* on_stream) const {
+        using MS = detail::MotionShader<T, Shader>;
+        check_motion_triangles("trace_triangles (motion)", motion);
+        triangle_batch<IsAnyHit, IsRobust, TieLastVisited>("trace_triangles (motion)", n,
+                                                           detail::TriangleShader<T, MS> { MS { shader }, motion, prim_ids },
+                                                           workspace, workspace_bytes, on_stream);
     }
 
     // Whole paths of triangle-ray segments, each continued in place from the last: see "Whole paths" at the top of this
@@ -1819,27 +1991,23 @@ template <typename T> struct DeviceView {
     void trace_paths(size_t n, const Shader& shader, void* workspace, size_t workspace_bytes, void* on_stream) const {
         if (!tris)
             throw std::invalid_argument("bvh::v2::cuda::DeviceView::trace_paths: the tree has no triangles (built from boxes)");
-        const bvhb200::TracePlan plan = batch_plan<false, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
-        const detail::TriangleShader<T, Shader> ts { shader, tris, prim_ids };
-#if defined(__CUDACC__)
-        run_batch("trace_paths", device_view_path_kernel<T, IsRobust, TieLastVisited, Shader>, ts, n, plan.refill_min,
-                  plan.inner_budget, workspace, workspace_bytes, on_stream);
-#else
-        (void)on_stream; (void)plan;
-        batch_stack_bytes("trace_paths", workspace, workspace_bytes);
-        using Payload = typename Shader::Payload;
-        for (size_t i = 0; i < n; ++i) {
-            Payload payload;
-            Ray ray;
-            PathStep step = shader.start(i, payload, ray);
-            while (step != PathStep::End) {
-                const Hit hit = step == PathStep::Occlusion ? host_triangle_ray<true, IsRobust, TieLastVisited>(ts, payload, ray)
-                                                            : host_triangle_ray<false, IsRobust, TieLastVisited>(ts, payload, ray);
-                step = shader.next(i, payload, hit, ray);
-            }
-            shader.finish(i, static_cast<const Payload&>(payload));
-        }
-#endif
+        path_batch<IsRobust, TieLastVisited>("trace_paths", n, detail::TriangleShader<T, Shader> { shader, tris, prim_ids }, workspace,
+                                             workspace_bytes, on_stream);
+    }
+    // The same through a mesh whose vertices move over the shutter, each path at its own time: see "Deforming meshes" at
+    // the top of this file.  The shader's start also gives the path's time, which holds for all its segments.
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_paths(size_t n, const MotionTriangles<T>& motion, const Shader& shader, void* workspace, size_t workspace_bytes) const {
+        trace_paths<IsRobust, TieLastVisited>(n, motion, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_paths(size_t n, const MotionTriangles<T>& motion, const Shader& shader, void* workspace, size_t workspace_bytes,
+                     void* on_stream) const {
+        using MS = detail::MotionShader<T, Shader>;
+        check_motion_triangles("trace_paths (motion)", motion);
+        path_batch<IsRobust, TieLastVisited>("trace_paths (motion)", n, detail::TriangleShader<T, MS> { MS { shader }, motion, prim_ids },
+                                             workspace, workspace_bytes, on_stream);
     }
 
     // A whole batch of triangle rays through a top-level tree of placed meshes: see "Instanced scenes" at the top of this
@@ -1931,6 +2099,62 @@ private:
         request.is_float = sizeof(T) == 4;
         request.n = n;
         return bvhb200::plan_trace(request);
+    }
+
+    // trace_triangles of either triangle source (`ts` holds the tree's triangles, or the keys of a deforming mesh with the
+    // shader wrapped in detail::MotionShader), named `call` in its errors.
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited, typename Shader>
+    void triangle_batch(const char* call, size_t n, const detail::TriangleShader<T, Shader>& ts, void* workspace, size_t workspace_bytes,
+                        void* on_stream) const {
+        const bvhb200::TracePlan plan = batch_plan<IsAnyHit, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
+#if defined(__CUDACC__)
+        run_batch(call, device_view_triangle_kernel<T, IsAnyHit, IsRobust, TieLastVisited, Shader>, ts, n, plan.refill_min,
+                  plan.inner_budget, workspace, workspace_bytes, on_stream);
+#else
+        (void)on_stream; (void)plan;
+        batch_stack_bytes(call, workspace, workspace_bytes);
+        using Payload = typename Shader::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            const Ray ray = ts.shader.start(i, payload);
+            ts.shader.finish(i, static_cast<const Payload&>(payload), host_triangle_ray<IsAnyHit, IsRobust, TieLastVisited>(ts, payload, ray));
+        }
+#endif
+    }
+
+    // trace_paths of either triangle source, as triangle_batch
+    template <bool IsRobust, bool TieLastVisited, typename Shader>
+    void path_batch(const char* call, size_t n, const detail::TriangleShader<T, Shader>& ts, void* workspace, size_t workspace_bytes,
+                    void* on_stream) const {
+        const bvhb200::TracePlan plan = batch_plan<false, IsRobust>(n, TieLastVisited ? bvhb200::kTraceLastVisited : 0u);
+#if defined(__CUDACC__)
+        run_batch(call, device_view_path_kernel<T, IsRobust, TieLastVisited, Shader>, ts, n, plan.refill_min, plan.inner_budget,
+                  workspace, workspace_bytes, on_stream);
+#else
+        (void)on_stream; (void)plan;
+        batch_stack_bytes(call, workspace, workspace_bytes);
+        using Payload = typename Shader::Payload;
+        for (size_t i = 0; i < n; ++i) {
+            Payload payload;
+            Ray ray;
+            PathStep step = ts.shader.start(i, payload, ray);
+            while (step != PathStep::End) {
+                const Hit hit = step == PathStep::Occlusion ? host_triangle_ray<true, IsRobust, TieLastVisited>(ts, payload, ray)
+                                                            : host_triangle_ray<false, IsRobust, TieLastVisited>(ts, payload, ray);
+                step = ts.shader.next(i, payload, hit, ray);
+            }
+            ts.shader.finish(i, static_cast<const Payload&>(payload));
+        }
+#endif
+    }
+
+    // The keys of the motion forms of trace_triangles and trace_paths: one triangle per primitive of this tree, both keys
+    void check_motion_triangles(const char* call, const MotionTriangles<T>& motion) const {
+        const std::string who = std::string("bvh::v2::cuda::DeviceView::") + call;
+        if (!motion.vertices[0] || !motion.vertices[1]) throw std::invalid_argument(who + ": a null key pointer");
+        if (motion.count != prim_count)
+            throw std::invalid_argument(who + ": " + std::to_string(motion.count) + " triangles for a tree of " +
+                                        std::to_string(prim_count) + " primitives");
     }
 
     // trace_instances of either record kind (Records: Instances<T> or MotionInstances<T>; `is` holds its records and the
@@ -2212,6 +2436,31 @@ void prepare_motion_instances(const MotionInstances<T>& instances, typename deta
 #else
     (void)stream;
     for (size_t i = 0; i < instances.count; ++i) detail::prepare_motion_instance<T>(instances.records[i], bboxes[i], centers[i]);
+#endif
+}
+
+// For every triangle of a deforming mesh (one thread each, stream-ordered on `stream`, no host synchronisation): in
+// bboxes[id] / centers[id] (device arrays of tris.count, original order) a box that holds triangle_at(tris, id, tau) at
+// every tau of the shutter, and the centre of the triangle at 0.5, ready for bvhNN_build_boxes or bvhNN_refit_boxes with
+// BVH_DEVICE_POINTERS.  See detail::prepare_motion_triangle for the bound; with equal keys, box and centre are
+// tri_bounds_center's of the key bit for bit.  A key with a non-finite entry gives an empty box.  The current device must
+// be the keys'.  A null pointer throws std::invalid_argument, a failed launch std::runtime_error.  Compiled as plain host
+// C++, the triangles are prepared serially.
+template <typename T>
+void prepare_motion_triangles(const MotionTriangles<T>& tris, typename detail::ViewTypes<T>::BBox* bboxes,
+                              typename detail::ViewTypes<T>::Vec* centers, void* stream = nullptr) {
+    if (tris.count == 0) return;
+    if (!tris.vertices[0] || !tris.vertices[1] || !bboxes || !centers)
+        throw std::invalid_argument("bvh::v2::cuda::prepare_motion_triangles: null keys, boxes or centres");
+#if defined(__CUDACC__)
+    const unsigned block = 128, grid = (unsigned)((tris.count + block - 1) / block);
+    prepare_motion_triangles_kernel<T><<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(tris, bboxes, centers);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess)
+        throw std::runtime_error(std::string("bvh::v2::cuda::prepare_motion_triangles: launch: ") + cudaGetErrorString(e));
+#else
+    (void)stream;
+    for (size_t i = 0; i < tris.count; ++i) detail::prepare_motion_triangle<T>(tris, i, bboxes[i], centers[i]);
 #endif
 }
 
