@@ -84,6 +84,8 @@ MOTION_INSTANCE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_motion_instanc
 MOTION_INSTANCE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_motion_instance_kernels.so")
 MOTION_TRIANGLE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_motion_triangle_kernels.cu")
 MOTION_TRIANGLE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_motion_triangle_kernels.so")
+MOTION_NODES_KERNELS_SRC = os.path.join(ROOT, "tests", "device_motion_nodes_kernels.cu")
+MOTION_NODES_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_motion_nodes_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -182,6 +184,13 @@ def build_device_motion_triangle_tests(force: bool = False, verbose: bool = Fals
     by hand one thread each, a path tracer with a time per path as one call, as a wavefront loop and as the static call,
     the benchmark's plain shader and traversal counts)."""
     return _build_test_kernels(MOTION_TRIANGLE_KERNELS_SRC, MOTION_TRIANGLE_KERNELS_LIB, force, verbose)
+
+
+def build_device_motion_nodes_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_motion_nodes_kernels.cu: the test shaders of prepare_motion_nodes, node_at and the motion-node forms
+    of DeviceView::trace_triangles and trace_paths (the deforming-mesh recording shader and path tracer, one thread per
+    ray through a node_at node test, subtree extents for containment, the benchmark's plain shader)."""
+    return _build_test_kernels(MOTION_NODES_KERNELS_SRC, MOTION_NODES_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

@@ -558,6 +558,52 @@
 //     bvh3f_refit_boxes(bvh, d_boxes, count, BVH_DEVICE_POINTERS);   // on the handle's stream (first frame: build_boxes)
 //     view.trace_triangles<false, false>(n, mesh, Shade { d_rays, d_times, d_hits }, workspace, bytes, stream);
 //
+// Motion nodes: the shutter boxes above hold each triangle over its whole sweep, so a mesh that moves a few triangle sizes
+// per shutter makes every ray test several times as many triangles.  Motion nodes keep the view's topology and give
+// each node its box at both keys: MotionNode<T> (per slot of the view's numbering, slot 0 unused: the bounds at key 0
+// and key 1 and the view's packed index; 64 bytes in float, 128 in double, so a sibling pair is one aligned 128 / 256-byte
+// block) and MotionNodes<T> { nodes, node_count } viewing view.node_count + 1 records in device memory.
+// node_at(motion_nodes, slot, time, bounds) is the one definition of a node's box at a time: each bound blended by
+// triangle_at's rule (detail::blend_key at detail::shutter_time(time)), so a bound that does not move is the key's own
+// bit for bit.  prepare_motion_nodes(view, motion_tris, out, workspace, bytes[, stream]) writes every record in one
+// view.traverse_bottom_up pass (workspace: view.bottom_up_workspace_bytes()): a leaf's key k is the union of
+// tri_bounds_center's boxes of its finite triangles at key k (refit_from_leaf's fold), widened on an axis on which
+// something moves by 4 eps M + the smallest normal number for the rounding of the two blends (triangle_at's and
+// node_at's; detail::MotionNodeBuilder states the bound); an inner node's keys are the unions of its children's, and a
+// side of it whose keys differ over a child whose keys on that side are equal (a static part beside a moving one) is
+// widened by the same rule.  So node_at's box of every node holds triangle_at of every finite triangle of its subtree at
+// every time.  With equal keys nothing is widened and both keys are the view's bounds after bvhNN_refit_boxes over
+// prepare_motion_triangles' boxes, bit for bit.
+// On that view:
+//     view.trace_triangles<IsAnyHit, IsRobust, TieLastVisited = false>(n, motion_tris, motion_nodes, shader, workspace, bytes[, stream]);
+//     view.trace_paths<IsRobust, TieLastVisited = false>(n, motion_tris, motion_nodes, shader, workspace, bytes[, stream]);
+// take the shaders of the motion forms (start also gives the time):
+//   * per ray (segment), the calls are exactly those of the motion form on a tree of the same topology whose node boxes
+//     are node_at(motion_nodes, slot, time): the same accept calls in the same order, the same record and, for paths,
+//     the same next calls.  With equal keys (one pointer twice) the call is the motion form on the shutter-box tree bit
+//     for bit, accept sequence included.  With moving keys whose entries are all finite, robust traversal and the
+//     canonical tie rule, closest-hit records equal the motion form's on every ray: both trees hold the closest
+//     triangle, only the visits differ.  (A triangle with a non-finite key is in neither tree's boxes, but a ray that
+//     reaches its leaf for a neighbour tests it, and the two trees reach different leaves.);
+//   * the view's node bounds are not read: its indices, prim_ids and depth are (the root index and the stack bound
+//     come from the motion nodes and view.depth);
+//   * errors, checked on the host before any launch: motion_nodes.node_count other than the view's, a null motion-node
+//     pointer, or the motion form's errors throw std::invalid_argument; a small workspace or a stack beyond 200 KB
+//     std::length_error; a failed launch std::runtime_error; the messages name "trace_triangles (motion nodes)" or
+//     "trace_paths (motion nodes)".  Streams, the workspace, n == 0, the warp subset and the host build are the motion
+//     form's; compiled as plain host C++, each ray runs traverse_top_down's loop with the same inner step;
+//   * the kernels are the motion forms' (device_view_triangle_kernel, device_view_path_kernel) with the shader wrapped
+//     as detail::MotionShader<T, detail::WithMotionNodes<T, Shader>>; the one step that differs is the inner step
+//     (detail::motion_inner_step): per child node_at's blend at the lane's time, then node_test's slab arithmetic and
+//     descend, unchanged, with float closest-hit rays splitting the fetch as inner_step does (x / y of both keys first,
+//     z and the index only for a child its x / y slabs do not reject).
+// One frame (the topology built once from the first frame's prepare_motion_triangles boxes):
+//
+//     skin<<<...>>>(d_key0, d_key1);
+//     prepare_motion_nodes(view, mesh, d_motion_nodes, bottom_up, view.bottom_up_workspace_bytes(), stream);
+//     view.trace_triangles<false, false>(n, mesh, MotionNodes<float> { d_motion_nodes, view.node_count }, Shade { ... },
+//                                        workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -639,6 +685,27 @@ template <typename T> struct MotionInstances {
 template <typename T> struct MotionTriangles {
     const T* vertices[2] = { nullptr, nullptr };
     size_t count = 0;
+};
+
+// The node of a deforming mesh's tree at the two keys, for the motion-node forms of trace_triangles and trace_paths: per
+// slot of a DeviceView's numbering (slot = reference index + 1, slot 0 unused) the node's bounds at time 0 and at time
+// 1 and its packed index, copied from the view, so that a traversal reads this array alone.  Key k's bounds are
+// minx, maxx, miny, maxy = xy[k][0..3] and minz, maxz = z[k][0..1].  64 bytes in float, 128 in double, so that a sibling
+// pair (slots 2j, 2j + 1) is one aligned 128 / 256-byte block of an array from cudaMalloc; in float the first 32 bytes
+// hold x and y of both keys and the second z of both keys and the index, the halves of the closest-hit step's split load.
+// prepare_motion_nodes writes them; node_at gives the box a ray of a given time tests.
+template <typename T> struct alignas(16 * sizeof(T)) MotionNode {
+    T xy[2][4];                         // key k: minx, maxx, miny, maxy
+    T z[2][2];                          // key k: minz, maxz
+    typename bvhb200::Real<T>::UInt index;          // the view's packed index of this slot
+    typename bvhb200::Real<T>::UInt pad[3];
+};
+static_assert(sizeof(MotionNode<float>) == 64 && sizeof(MotionNode<double>) == 128, "motion node size");
+
+// A plain view of the node_count + 1 motion nodes of a tree (slot 0 unused) in device memory.
+template <typename T> struct MotionNodes {
+    const MotionNode<T>* nodes = nullptr;
+    size_t node_count = 0;
 };
 
 namespace detail {
@@ -867,6 +934,59 @@ template <typename T> BVH_HD T load_key(const T* p) {
     return *p;
 #endif
 }
+
+// The halves of a motion node, read through the read-only cache on the device: x and y of both keys (the first 32 bytes
+// in float, two 128-bit loads), and z of both keys with the index (one 128-bit load and one 32-bit load in float).
+#if defined(__CUDA_ARCH__)
+__device__ __forceinline__ void load_motion_xy(const MotionNode<float>* p, float (&xy)[2][4]) {
+    const float4* q = reinterpret_cast<const float4*>(p);
+    const float4 a = __ldg(q), b = __ldg(q + 1);
+    xy[0][0] = a.x; xy[0][1] = a.y; xy[0][2] = a.z; xy[0][3] = a.w;
+    xy[1][0] = b.x; xy[1][1] = b.y; xy[1][2] = b.z; xy[1][3] = b.w;
+}
+__device__ __forceinline__ void load_motion_z(const MotionNode<float>* p, float (&z)[2][2], uint32_t& index) {
+    const float4 c = __ldg(reinterpret_cast<const float4*>(p) + 2);
+    z[0][0] = c.x; z[0][1] = c.y; z[1][0] = c.z; z[1][1] = c.w;
+    index = __ldg(&p->index);
+}
+__device__ __forceinline__ void load_motion_xy(const MotionNode<double>* p, double (&xy)[2][4]) {
+    const double2* q = reinterpret_cast<const double2*>(p);
+    #pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const double2 a = __ldg(q + k);
+        xy[k / 2][2 * (k % 2)] = a.x; xy[k / 2][2 * (k % 2) + 1] = a.y;
+    }
+}
+__device__ __forceinline__ void load_motion_z(const MotionNode<double>* p, double (&z)[2][2], uint64_t& index) {
+    const double2* q = reinterpret_cast<const double2*>(p) + 4;
+    const double2 a = __ldg(q), b = __ldg(q + 1);
+    z[0][0] = a.x; z[0][1] = a.y; z[1][0] = b.x; z[1][1] = b.y;
+    index = (uint64_t)__ldg(reinterpret_cast<const unsigned long long*>(&p->index));
+}
+#else
+template <typename T> inline void load_motion_xy(const MotionNode<T>* p, T (&xy)[2][4]) {
+    for (int k = 0; k < 2; ++k)
+        for (int q = 0; q < 4; ++q) xy[k][q] = p->xy[k][q];
+}
+template <typename T> inline void load_motion_z(const MotionNode<T>* p, T (&z)[2][2], typename bvhb200::Real<T>::UInt& index) {
+    for (int k = 0; k < 2; ++k) { z[k][0] = p->z[k][0]; z[k][1] = p->z[k][1]; }
+    index = p->index;
+}
+#endif
+// The bounds of the motion node at p blended to (tau, rest) by blend_key: x and y into b[0..3], z into b[4..5] (and the
+// node's index).  node_at and the inner step of the motion-node forms both blend through these.
+template <typename T> BVH_HD void blend_node_xy(const MotionNode<T>* p, T tau, T rest, T* b) {
+    T xy[2][4];
+    load_motion_xy(p, xy);
+    for (int q = 0; q < 4; ++q) b[q] = blend_key(xy[0][q], xy[1][q], tau, rest);
+}
+template <typename T>
+BVH_HD void blend_node_z(const MotionNode<T>* p, T tau, T rest, T* b, typename bvhb200::Real<T>::UInt& index) {
+    T z[2][2];
+    load_motion_z(p, z, index);
+    b[4] = blend_key(z[0][0], z[1][0], tau, rest);
+    b[5] = blend_key(z[0][1], z[1][1], tau, rest);
+}
 }
 
 // Triangle `id` of a deforming mesh at `time` (both builds), its three vertices p0, p1, p2 into v: each coordinate
@@ -882,6 +1002,20 @@ template <typename T> BVH_HD void triangle_at(const MotionTriangles<T>& tris, si
     const T* k0 = tris.vertices[0] + 9 * id;
     const T* k1 = tris.vertices[1] + 9 * id;
     for (int k = 0; k < 9; ++k) v[k] = detail::blend_key(detail::load_key(k0 + k), detail::load_key(k1 + k), tau, rest);
+}
+
+// The box of motion node `slot` at `time` (both builds), minx, maxx, miny, maxy, minz, maxz into bounds: each bound
+// blended from the node's two keys by triangle_at's rule (detail::blend_key with tau = detail::shutter_time(time): time
+// clamped to [0, 1], a NaN time as 0; exact at 0 and 1 and for bounds whose keys agree, so a bound that does not move is
+// the key's own bit for bit).  The motion-node forms of trace_triangles and trace_paths test a ray of that time against
+// exactly this box with the library's slab test.  On the device it reads the node through the read-only cache.
+template <typename T> BVH_HD void node_at(const MotionNodes<T>& motion_nodes, size_t slot, T time, T bounds[6]) {
+    using R = bvhb200::Real<T>;
+    const T tau = detail::shutter_time(time);
+    const T rest = R::sub(T(1), tau);
+    typename R::UInt index;
+    detail::blend_node_xy(motion_nodes.nodes + slot, tau, rest, bounds);
+    detail::blend_node_z(motion_nodes.nodes + slot, tau, rest, bounds, index);
 }
 
 namespace detail {
@@ -933,6 +1067,150 @@ BVH_HD void prepare_motion_triangle(const MotionTriangles<T>& tris, size_t id, t
     box.max.x = hi[0]; box.max.y = hi[1]; box.max.z = hi[2];
     centre.x = mid[0]; centre.y = mid[1]; centre.z = mid[2];
 }
+
+// A sibling's motion node was written by another thread (another SM on the device): read it through L2, as
+// refit_load_child reads a refitted node.
+template <typename T> BVH_HD MotionNode<T> load_motion_child(const MotionNode<T>* p) {
+#if defined(__CUDA_ARCH__)
+    MotionNode<T> out;
+    const uint4* s = reinterpret_cast<const uint4*>(p);
+    uint4* d = reinterpret_cast<uint4*>(&out);
+    #pragma unroll
+    for (int k = 0; k < (int)(sizeof(MotionNode<T>) / 16); ++k) d[k] = __ldcg(s + k);
+    return out;
+#else
+    return *p;
+#endif
+}
+
+// prepare_motion_nodes' leaf and inner functions for DeviceView::traverse_bottom_up (both builds): motion node `node`
+// (a reference index; its record is out[node + 1]) from the two vertex keys.
+//   * leaf: per key, the union of tri_bounds_center's boxes of the leaf's triangles at that key, in BVH order, with
+//     robust_min / robust_max from +-max (refit_from_leaf's fold, so with equal keys both keys are the refitted bounds
+//     of prepare_motion_triangles' boxes bit for bit).  A triangle with a non-finite key adds nothing to either key;
+//   * then each side of an axis on which some coordinate of the leaf's triangles moves is moved out, at both keys, by
+//     d = 4 eps M + the smallest normal number, M the largest magnitude of the axis' four unwidened bounds;
+//   * inner: per key, the union of its children's records (left first, as refit_from_leaf), read through L2; then a side
+//     whose two keys differ while a child's two keys on it are equal is moved out at both keys by d, M now the largest
+//     magnitude of the node's four bounds on that axis;
+//   * the index is the view's; a node that holds nothing keeps +-max at both keys, which node_at returns exactly and
+//     the slab test misses at every time.
+// Why node_at(node, tau) holds triangle_at of every finite triangle of the subtree (the lower side of an axis; the upper
+// is symmetric).  node_at and triangle_at blend with the same weights tau and rest = fl(1 - tau), both >= 0, and each
+// blend_key of keys k0, k1 is within eps (rest |k0| + tau |k1|) (1 + O(eps)) of the exact weighted sum rest k0 + tau k1
+// (two products and a sum, each within eps/2; the exact branches within eps/2 |k|, as rest + tau is within eps/2 of 1).
+// So a node bound P blends to at most G(P) = rest F(P0) + tau F(P1) and a coordinate c to at least
+// rest F-(c0) + tau F-(c1), F(x) = x + eps |x| (1 + O(eps)) and F-(x) = x - eps |x| (1 + O(eps)) both increasing: a node
+// bound further out only moves its bound on the blend further out.  Each node side keeps one of two invariants:
+//   (E) its two keys are equal: node_at returns the key P exactly.  A coordinate that does not move blends to itself,
+//       and lies at or inside P.  One that moves lies in a widened leaf, d inside P at both keys, and its blend loses at
+//       most eps M (1 + O(eps)) of that;
+//   (W) its keys differ, and every coordinate of the subtree lies at least a widening d (of a node at or below this
+//       one, whose M is at least the coordinate's magnitude or whose bound is further out by more than the excess) inside
+//       the node's bound at both keys.  A leaf whose keys differ has a moving axis, so it was widened.  An inner node
+//       keeps (W) from a child that has it (its own bound is the union, further out), and takes it from a child with
+//       equal keys by its own widening: without that, rest P + tau (P - e) for a static coordinate P of that child can
+//       round to one ulp beyond P when rest + tau > 1.
+//   Under (W) the two blends lose at most 2 eps M + eps d and the rounding of the widened bound takes back at most
+//   eps/2 (M + d): 2.5 eps M + 1.5 eps d < d.  (The 3 eps M of prepare_motion_triangle covers one rounded blend, not two.)
+// With equal keys nothing moves, no side is widened, and every record is the refitted bound bit for bit.  A bound is
+// widened once per level at most where static and moving parts of the mesh meet under it, so at most depth x d.
+template <typename T> struct MotionNodeBuilder {
+    const bvhb200::DevNode<T>* nodes;   // the view's nodes: only their packed indices are read
+    const uint32_t* prim_ids;
+    MotionTriangles<T> tris;
+    MotionNode<T>* out;
+
+    BVH_HD void operator()(size_t node, size_t begin, size_t end) const {
+        using R = bvhb200::Real<T>;
+        const T pad = R::mul(R::eps(), T(4)), tiny = sizeof(T) == 4 ? (T)FLT_MIN : (T)DBL_MIN;
+        T lo[2][3], hi[2][3];
+        bool moves[3] = { false, false, false };
+        for (int k = 0; k < 2; ++k)
+            for (int a = 0; a < 3; ++a) { lo[k][a] = R::max(); hi[k][a] = R::neg(R::max()); }
+        for (size_t slot = begin; slot < end; ++slot) {
+            const size_t id = prim_ids[slot];
+            T v[2][9];
+            bool ok = true;
+            for (int q = 0; q < 9; ++q) {
+                v[0][q] = load_key(tris.vertices[0] + 9 * id + q);
+                v[1][q] = load_key(tris.vertices[1] + 9 * id + q);
+                ok = ok && R::is_finite(v[0][q]) && R::is_finite(v[1][q]);
+            }
+            if (!ok) continue;
+            for (int k = 0; k < 2; ++k) {
+                T bmin[3], bmax[3], c[3];
+                bvhb200::tri_bounds_center(v[k], bmin, bmax, c);
+                for (int a = 0; a < 3; ++a) {
+                    lo[k][a] = bvhb200::robust_min(lo[k][a], bmin[a]);
+                    hi[k][a] = bvhb200::robust_max(hi[k][a], bmax[a]);
+                }
+            }
+            for (int a = 0; a < 3; ++a)
+                moves[a] = moves[a] || v[0][a] != v[1][a] || v[0][3 + a] != v[1][3 + a] || v[0][6 + a] != v[1][6 + a];
+        }
+        for (int a = 0; a < 3; ++a) {
+            if (!moves[a]) continue;
+            T m = T(0);
+            for (int k = 0; k < 2; ++k) {
+                m = m < R::abs(lo[k][a]) ? R::abs(lo[k][a]) : m;
+                m = m < R::abs(hi[k][a]) ? R::abs(hi[k][a]) : m;
+            }
+            const T d = R::add(R::mul(m, pad), tiny);
+            for (int k = 0; k < 2; ++k) { lo[k][a] = R::sub(lo[k][a], d); hi[k][a] = R::add(hi[k][a], d); }
+        }
+        write(node, lo, hi);
+    }
+
+    BVH_HD void operator()(size_t node, size_t left) const {
+        const MotionNode<T> l = load_motion_child(out + left + 1), r = load_motion_child(out + left + 2);
+        T lo[2][3], hi[2][3];
+        for (int k = 0; k < 2; ++k) {
+            for (int a = 0; a < 2; ++a) {
+                lo[k][a] = bvhb200::robust_min(l.xy[k][2 * a], r.xy[k][2 * a]);
+                hi[k][a] = bvhb200::robust_max(l.xy[k][2 * a + 1], r.xy[k][2 * a + 1]);
+            }
+            lo[k][2] = bvhb200::robust_min(l.z[k][0], r.z[k][0]);
+            hi[k][2] = bvhb200::robust_max(l.z[k][1], r.z[k][1]);
+        }
+        // a side whose keys differ over a child side whose keys are equal (a part that does not move): moved out by d
+        using R = bvhb200::Real<T>;
+        const T pad = R::mul(R::eps(), T(4)), tiny = sizeof(T) == 4 ? (T)FLT_MIN : (T)DBL_MIN;
+        auto side = [](const MotionNode<T>& c, int k, int a, int hi_side) {
+            return a < 2 ? c.xy[k][2 * a + hi_side] : c.z[k][hi_side];
+        };
+        for (int a = 0; a < 3; ++a) {
+            bool widen[2];
+            for (int h = 0; h < 2; ++h) {
+                const T* key = h ? &hi[0][a] : &lo[0][a];           // key k at key[3 k]
+                widen[h] = key[0] != key[3] && (side(l, 0, a, h) == side(l, 1, a, h) || side(r, 0, a, h) == side(r, 1, a, h));
+            }
+            if (!widen[0] && !widen[1]) continue;
+            T m = T(0);
+            for (int k = 0; k < 2; ++k) {
+                m = m < R::abs(lo[k][a]) ? R::abs(lo[k][a]) : m;
+                m = m < R::abs(hi[k][a]) ? R::abs(hi[k][a]) : m;
+            }
+            const T d = R::add(R::mul(m, pad), tiny);
+            for (int k = 0; k < 2; ++k) {
+                if (widen[0]) lo[k][a] = R::sub(lo[k][a], d);
+                if (widen[1]) hi[k][a] = R::add(hi[k][a], d);
+            }
+        }
+        write(node, lo, hi);
+    }
+
+    BVH_HD void write(size_t node, const T (&lo)[2][3], const T (&hi)[2][3]) const {
+        MotionNode<T> o;
+        for (int k = 0; k < 2; ++k) {
+            for (int a = 0; a < 2; ++a) { o.xy[k][2 * a] = lo[k][a]; o.xy[k][2 * a + 1] = hi[k][a]; }
+            o.z[k][0] = lo[k][2]; o.z[k][1] = hi[k][2];
+        }
+        o.index = nodes[node + 1].index;
+        o.pad[0] = o.pad[1] = o.pad[2] = 0;
+        out[node + 1] = o;
+    }
+};
 
 // prepare_motion_instances for one record (both builds).  root_index: the bottom root's.  The box holds the bottom
 // root box at every time of the shutter, under the placement blend_keys computes:
@@ -1041,6 +1319,57 @@ BVH_HD void shader_leaf(const TriangleShader<T, MotionShader<T, Shader>>& ts, Pa
             return ts.shader.accept(payload, static_cast<size_t>(id), t, u, w);
         });
     }
+}
+
+// The caller's shader of the motion-node forms of trace_triangles and trace_paths with the tree's motion nodes beside
+// it.  It runs wrapped in MotionShader, like the shader of the motion forms, so the leaf, the record and the time are
+// theirs; the kernels see the motion nodes through HasMotionNodes and take motion_inner_step instead of inner_step.
+template <typename T, typename Shader> struct WithMotionNodes {
+    using Payload = typename Shader::Payload;
+    Shader shader;
+    MotionNodes<T> motion_nodes;
+    template <typename... A> BVH_HD decltype(auto) start(A&&... a) const { return shader.start(std::forward<A>(a)...); }
+    template <typename... A> BVH_HD decltype(auto) accept(A&&... a) const { return shader.accept(std::forward<A>(a)...); }
+    template <typename... A> BVH_HD decltype(auto) next(A&&... a) const { return shader.next(std::forward<A>(a)...); }
+    template <typename... A> BVH_HD void finish(A&&... a) const { shader.finish(std::forward<A>(a)...); }
+};
+// Whether a triangle kernel's shader carries motion nodes
+template <typename Shader> struct HasMotionNodes : std::false_type {};
+template <typename T, typename Shader> struct HasMotionNodes<MotionShader<T, WithMotionNodes<T, Shader>>> : std::true_type {};
+
+// The inner step of the motion-node forms (both builds): inner_step with each child's box blended to the ray's time.
+// Per child, node_at's blend (blend_node_xy, blend_node_z) at tau = shutter_time(time), then node_test's slab arithmetic
+// and descend, unchanged.  Float closest-hit rays split the fetch as inner_step does: x and y of both keys of both
+// children first (two 32-byte halves), and z and the index of a child only when its x / y interval is not already
+// empty, with the same operations in the same order as node_test.  Any-hit and double-precision rays read whole nodes.
+template <typename T, bool kAny, bool kRobust, typename Stack>
+BVH_HD void motion_inner_step(const MotionNode<T>* __restrict__ nodes, T time, const bvhb200::RayCtx<T>& r,
+                              typename bvhb200::Real<T>::UInt& top, Stack& stack) {
+    using R = bvhb200::Real<T>;
+    using U = typename R::UInt;
+    const T tau = shutter_time(time);
+    const T rest = R::sub(T(1), tau);
+    const MotionNode<T>* p = nodes + 1 + bvhb200::index_first(top);       // the left child's slot
+    T lb[6], rb[6];
+    U li = 0, ri = 0;
+    T l0 = r.tmin, l1 = r.tmax, r0 = r.tmin, r1 = r.tmax;
+    if constexpr (sizeof(T) == 4 && !kAny) {
+        blend_node_xy(p, tau, rest, lb);
+        blend_node_xy(p + 1, tau, rest, rb);
+        bvhb200::node_test_axes<T, kRobust, 0, 2>(lb, r, l0, l1);
+        bvhb200::node_test_axes<T, kRobust, 0, 2>(rb, r, r0, r1);
+        if (l0 <= l1) { blend_node_z(p, tau, rest, lb, li); bvhb200::node_test_axes<T, kRobust, 2, 3>(lb, r, l0, l1); }
+        if (r0 <= r1) { blend_node_z(p + 1, tau, rest, rb, ri); bvhb200::node_test_axes<T, kRobust, 2, 3>(rb, r, r0, r1); }
+    } else {
+        blend_node_xy(p, tau, rest, lb);
+        blend_node_z(p, tau, rest, lb, li);
+        blend_node_xy(p + 1, tau, rest, rb);
+        blend_node_z(p + 1, tau, rest, rb, ri);
+        bvhb200::node_test<T, kRobust>(lb, r, l0, l1);
+        bvhb200::node_test<T, kRobust>(rb, r, r0, r1);
+    }
+    // ties go left first, as in inner_step
+    bvhb200::descend<U>(l0 <= l1, r0 <= r1, !kAny && l0 > r0, li, ri, top, stack);
 }
 
 // The placement a ray meets a record at, as its world_to_object handed to f (both builds): a static record's own; for
@@ -1395,19 +1724,23 @@ device_view_triangle_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsig
             hit.slot = bvhb200::kInvalidId; hit.t = r.tmax; hit.u = T(0); hit.v = T(0);
             if (bvhb200::ray_interval_is_nan(r)) { retire(); return; }
             bvhb200::ray_prologue<T, IsRobust>(r);
-            top = nodes[1].index;
+            if constexpr (detail::HasMotionNodes<Shader>::value) top = ts.shader.shader.motion_nodes.nodes[1].index;
+            else top = nodes[1].index;
             stack.clear();
             has_ray = true;
         });
     };
 
     // inner phase: descend until this lane holds a leaf, its ray is finished, or the step budget of this round is spent
+    // (with motion nodes, each child's box at the ray's time)
     auto inner = [&] {
         if (has_ray) {
             uint32_t budget = inner_budget;
             while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone ends it too)
                 --budget;
-                bvhb200::inner_step<T, IsAnyHit, IsRobust>(nodes, r, top, stack);
+                if constexpr (detail::HasMotionNodes<Shader>::value)
+                    detail::motion_inner_step<T, IsAnyHit, IsRobust>(ts.shader.shader.motion_nodes.nodes, payload.time, r, top, stack);
+                else bvhb200::inner_step<T, IsAnyHit, IsRobust>(nodes, r, top, stack);
             }
             if (top == bvhb200::kTraversalDone<U>) retire();
         }
@@ -1463,7 +1796,9 @@ device_view_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned 
         top = bvhb200::kTraversalDone<U>;
         if (!bvhb200::ray_interval_is_nan(r)) {
             bvhb200::ray_prologue<T, IsRobust>(r);
-            top = nodes[1].index;       // (read per segment, as device_view_triangle_kernel reads it per ray)
+            // (read per segment, as device_view_triangle_kernel reads it per ray)
+            if constexpr (detail::HasMotionNodes<Shader>::value) top = ts.shader.shader.motion_nodes.nodes[1].index;
+            else top = nodes[1].index;
         }
         stack.clear();
         has_path = true;
@@ -1494,8 +1829,14 @@ device_view_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsigned 
             uint32_t budget = inner_budget;
             while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone ends it too)
                 --budget;
-                if (occlusion) bvhb200::inner_step<T, true, IsRobust>(nodes, r, top, stack);
-                else bvhb200::inner_step<T, false, IsRobust>(nodes, r, top, stack);
+                if constexpr (detail::HasMotionNodes<Shader>::value) {
+                    const MotionNode<T>* motion_nodes = ts.shader.shader.motion_nodes.nodes;
+                    if (occlusion) detail::motion_inner_step<T, true, IsRobust>(motion_nodes, payload.time, r, top, stack);
+                    else detail::motion_inner_step<T, false, IsRobust>(motion_nodes, payload.time, r, top, stack);
+                } else {
+                    if (occlusion) bvhb200::inner_step<T, true, IsRobust>(nodes, r, top, stack);
+                    else bvhb200::inner_step<T, false, IsRobust>(nodes, r, top, stack);
+                }
             }
         }
     };
@@ -1979,6 +2320,26 @@ template <typename T> struct DeviceView {
                                                            detail::TriangleShader<T, MS> { MS { shader }, motion, prim_ids },
                                                            workspace, workspace_bytes, on_stream);
     }
+    // The same with the tree's motion nodes (prepare_motion_nodes): each inner step tests the children's boxes at the
+    // ray's time (node_at) instead of this view's boxes over the whole shutter.  See "Deforming meshes" at the top of
+    // this file.  The view's node bounds are not read.
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_triangles(size_t n, const MotionTriangles<T>& motion, const MotionNodes<T>& motion_nodes, const Shader& shader,
+                         void* workspace, size_t workspace_bytes) const {
+        trace_triangles<IsAnyHit, IsRobust, TieLastVisited>(n, motion, motion_nodes, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_triangles(size_t n, const MotionTriangles<T>& motion, const MotionNodes<T>& motion_nodes, const Shader& shader,
+                         void* workspace, size_t workspace_bytes, void* on_stream) const {
+        using MS = detail::MotionShader<T, detail::WithMotionNodes<T, Shader>>;
+        check_motion_triangles("trace_triangles (motion nodes)", motion);
+        check_motion_nodes("trace_triangles (motion nodes)", motion_nodes);
+        triangle_batch<IsAnyHit, IsRobust, TieLastVisited>(
+            "trace_triangles (motion nodes)", n,
+            detail::TriangleShader<T, MS> { MS { detail::WithMotionNodes<T, Shader> { shader, motion_nodes } }, motion, prim_ids },
+            workspace, workspace_bytes, on_stream);
+    }
 
     // Whole paths of triangle-ray segments, each continued in place from the last: see "Whole paths" at the top of this
     // file.  The workspace is the warps' run cursor, trace_workspace_bytes() bytes.
@@ -2008,6 +2369,24 @@ template <typename T> struct DeviceView {
         check_motion_triangles("trace_paths (motion)", motion);
         path_batch<IsRobust, TieLastVisited>("trace_paths (motion)", n, detail::TriangleShader<T, MS> { MS { shader }, motion, prim_ids },
                                              workspace, workspace_bytes, on_stream);
+    }
+    // The same with the tree's motion nodes (prepare_motion_nodes), as for trace_triangles.
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_paths(size_t n, const MotionTriangles<T>& motion, const MotionNodes<T>& motion_nodes, const Shader& shader, void* workspace,
+                     size_t workspace_bytes) const {
+        trace_paths<IsRobust, TieLastVisited>(n, motion, motion_nodes, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_paths(size_t n, const MotionTriangles<T>& motion, const MotionNodes<T>& motion_nodes, const Shader& shader, void* workspace,
+                     size_t workspace_bytes, void* on_stream) const {
+        using MS = detail::MotionShader<T, detail::WithMotionNodes<T, Shader>>;
+        check_motion_triangles("trace_paths (motion nodes)", motion);
+        check_motion_nodes("trace_paths (motion nodes)", motion_nodes);
+        path_batch<IsRobust, TieLastVisited>(
+            "trace_paths (motion nodes)", n,
+            detail::TriangleShader<T, MS> { MS { detail::WithMotionNodes<T, Shader> { shader, motion_nodes } }, motion, prim_ids },
+            workspace, workspace_bytes, on_stream);
     }
 
     // A whole batch of triangle rays through a top-level tree of placed meshes: see "Instanced scenes" at the top of this
@@ -2156,6 +2535,14 @@ private:
             throw std::invalid_argument(who + ": " + std::to_string(motion.count) + " triangles for a tree of " +
                                         std::to_string(prim_count) + " primitives");
     }
+    // The motion nodes of the motion-node forms: one record per slot of this tree
+    void check_motion_nodes(const char* call, const MotionNodes<T>& motion_nodes) const {
+        const std::string who = std::string("bvh::v2::cuda::DeviceView::") + call;
+        if (!motion_nodes.nodes) throw std::invalid_argument(who + ": a null motion-node pointer");
+        if (motion_nodes.node_count != node_count)
+            throw std::invalid_argument(who + ": motion nodes of " + std::to_string(motion_nodes.node_count) + " nodes for a tree of " +
+                                        std::to_string(node_count) + " nodes");
+    }
 
     // trace_instances of either record kind (Records: Instances<T> or MotionInstances<T>; `is` holds its records and the
     // shader, wrapped in detail::MotionShader for motion records), named `call` in its errors.
@@ -2231,13 +2618,28 @@ private:
             bvhb200::ray_prologue<T, IsRobust>(r);
             detail::VectorStack<Index> stack;
             stack.elems.reserve(stack_bound());
-            bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
-                nodes, r, root_index(), stack,
-                [&](Index begin, Index end) {
-                    detail::shader_leaf<T, TieLastVisited>(ts, payload, (uint32_t)begin, (uint32_t)(end - begin), r, hit);
-                    return hit.slot != bvhb200::kInvalidId;
-                },
-                [](Index) {});
+            if constexpr (detail::HasMotionNodes<Shader>::value) {
+                // traverse_top_down's loop with the inner step of the motion-node forms (the interval stays a number:
+                // a leaf only shrinks tmax to a hit's t)
+                const MotionNode<T>* motion_nodes = ts.shader.shader.motion_nodes.nodes;
+                Index top = motion_nodes[1].index;
+                for (;;) {
+                    while (bvhb200::index_count(top) == 0)
+                        detail::motion_inner_step<T, IsAnyHit, IsRobust>(motion_nodes, payload.time, r, top, stack);
+                    if (top == bvhb200::kTraversalDone<Index>) break;
+                    detail::shader_leaf<T, TieLastVisited>(ts, payload, (uint32_t)bvhb200::index_first(top), bvhb200::index_count(top), r, hit);
+                    if (IsAnyHit && hit.slot != bvhb200::kInvalidId) break;
+                    top = bvhb200::pop_or_done<Index>(stack);
+                }
+            } else {
+                bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
+                    nodes, r, root_index(), stack,
+                    [&](Index begin, Index end) {
+                        detail::shader_leaf<T, TieLastVisited>(ts, payload, (uint32_t)begin, (uint32_t)(end - begin), r, hit);
+                        return hit.slot != bvhb200::kInvalidId;
+                    },
+                    [](Index) {});
+            }
         }
         return detail::make_hit<T>(bvhb200::make_record(hit, tmax_in, prim_ids));
     }
@@ -2462,6 +2864,41 @@ void prepare_motion_triangles(const MotionTriangles<T>& tris, typename detail::V
     (void)stream;
     for (size_t i = 0; i < tris.count; ++i) detail::prepare_motion_triangle<T>(tris, i, bboxes[i], centers[i]);
 #endif
+}
+
+// The motion nodes of `view`'s topology for a deforming mesh (stream-ordered on `stream`, the view's by default, no host
+// synchronisation): into out[1 .. view.node_count] (a device array of view.node_count + 1 records; slot 0 is not
+// written) each node's bounds at time 0 and at time 1 from the two vertex keys, and its packed index, for the
+// motion-node forms of trace_triangles and trace_paths.  One pass of view.traverse_bottom_up (its two kernels, on
+// `workspace` of view.bottom_up_workspace_bytes() bytes); see detail::MotionNodeBuilder for the boxes and the widening
+// bound.  With equal keys both keys of every record are the view's node bounds after bvhNN_refit_boxes over
+// prepare_motion_triangles' boxes, bit for bit.  The topology is the view's: build it once (bvhNN_build_boxes over
+// prepare_motion_triangles' boxes) and call this once per frame.  A null pointer or a triangle count other than the
+// tree's throws std::invalid_argument, a small workspace std::length_error, a failed launch std::runtime_error, each
+// naming prepare_motion_nodes.  Compiled as plain host C++, the pass runs serially.
+template <typename T>
+void prepare_motion_nodes(const DeviceView<T>& view, const MotionTriangles<T>& tris, MotionNode<T>* out, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+    const std::string who = "bvh::v2::cuda::prepare_motion_nodes: ";
+    if (!tris.vertices[0] || !tris.vertices[1] || !out) throw std::invalid_argument(who + "null keys or motion nodes");
+    if (tris.count != view.prim_count)
+        throw std::invalid_argument(who + std::to_string(tris.count) + " triangles for a tree of " + std::to_string(view.prim_count) +
+                                    " primitives");
+    const size_t need = view.bottom_up_workspace_bytes();
+    if (workspace_bytes < need || !workspace)
+        throw std::length_error(who + "a workspace of " + std::to_string(workspace ? workspace_bytes : 0) + " bytes is too small for " +
+                                std::to_string(view.node_count) + " nodes (" + std::to_string(need) + " bytes)");
+    const detail::MotionNodeBuilder<T> builder { view.nodes, view.prim_ids, tris, out };
+    try {
+        view.traverse_bottom_up(workspace, workspace_bytes, builder, builder, stream);
+    } catch (const std::runtime_error& e) {
+        throw std::runtime_error(who + e.what());
+    }
+}
+template <typename T>
+void prepare_motion_nodes(const DeviceView<T>& view, const MotionTriangles<T>& tris, MotionNode<T>* out, void* workspace,
+                          size_t workspace_bytes) {
+    prepare_motion_nodes(view, tris, out, workspace, workspace_bytes, view.stream);
 }
 
 } // namespace bvh::v2::cuda
