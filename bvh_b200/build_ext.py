@@ -86,6 +86,8 @@ MOTION_TRIANGLE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_motion_triangl
 MOTION_TRIANGLE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_motion_triangle_kernels.so")
 MOTION_NODES_KERNELS_SRC = os.path.join(ROOT, "tests", "device_motion_nodes_kernels.cu")
 MOTION_NODES_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_motion_nodes_kernels.so")
+DEFORMING_INSTANCE_KERNELS_SRC = os.path.join(ROOT, "tests", "device_deforming_instance_kernels.cu")
+DEFORMING_INSTANCE_KERNELS_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_deforming_instance_kernels.so")
 
 
 def _build_test_kernels(src: str, out: str, force: bool, verbose: bool) -> str:
@@ -191,6 +193,14 @@ def build_device_motion_nodes_tests(force: bool = False, verbose: bool = False) 
     of DeviceView::trace_triangles and trace_paths (the deforming-mesh recording shader and path tracer, one thread per
     ray through a node_at node test, subtree extents for containment, the benchmark's plain shader)."""
     return _build_test_kernels(MOTION_NODES_KERNELS_SRC, MOTION_NODES_KERNELS_LIB, force, verbose)
+
+
+def build_device_deforming_instance_tests(force: bool = False, verbose: bool = False) -> str:
+    """tests/device_deforming_instance_kernels.cu: the test shaders of the deforming forms of DeviceView::trace_instances
+    and trace_instance_paths, make_deforming_instance and prepare_deforming_instances (a recording shader with a time
+    per ray, the same rays nested by hand one thread each, the motion and triangle calls they reduce to, scripted paths,
+    the benchmark's plain shader)."""
+    return _build_test_kernels(DEFORMING_INSTANCE_KERNELS_SRC, DEFORMING_INSTANCE_KERNELS_LIB, force, verbose)
 
 
 if __name__ == "__main__":

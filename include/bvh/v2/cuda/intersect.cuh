@@ -604,6 +604,42 @@
 //     view.trace_triangles<false, false>(n, mesh, MotionNodes<float> { d_motion_nodes, view.node_count }, Shade { ... },
 //                                        workspace, bytes, stream);
 //
+// Deforming instances: a scene that mixes static placed meshes with deforming ones (a skinned character among instanced
+// set pieces), in one launch.  A DeformingInstance<T> record holds MotionInstance<T>'s fields and a bottom's vertex keys
+// and motion nodes; DeformingInstances<T> { records, count, max_depth } views them.  Each record picks its bottom kind
+// at run time: vertices[0] == nullptr is a static bottom (the view's tris and node bounds); vertex keys alone are a
+// deforming bottom on the view's tree refitted over prepare_motion_triangles' boxes; vertex keys and motion nodes are a
+// deforming bottom whose inner steps are motion_inner_step at the ray's time.  make_deforming_instance(view, key0, key1
+// [, motion_tris[, motion_nodes]]) fills one on the host (std::invalid_argument for a count other than the view's or a
+// null pointer).  prepare_deforming_instances(instances, bboxes, centers[, stream]) writes every root index and a world
+// box that holds every finite triangle of the bottom at every time under the placement at that time
+// (detail::prepare_deforming_instance states the argument), after each deforming bottom's own step of the frame
+// (prepare_motion_triangles + bvhNN_refit_boxes, or prepare_motion_nodes).  On the top view:
+//     top.trace_instances<IsAnyHit, IsRobust, TieLastVisited = false>(n, deforming_instances, shader, workspace, bytes[, stream]);
+//     top.trace_instance_paths<IsRobust, TieLastVisited = false>(n, deforming_instances, shader, workspace, bytes[, stream]);
+// take the motion forms' shaders (start also gives the time):
+//   * per ray (segment), the calls are exactly those of the motion forms on the same top tree, except inside a record
+//     with a deforming bottom, whose bottom traversal is the motion trace_triangles (shutter boxes) or the motion-node
+//     trace_triangles at the ray's time on the object-space ray of instance_at(record, time); leaf ties take the
+//     canonical rule on (instance, original id) unless TieLastVisited;
+//   * so with static bottoms only the call is the motion trace_instances, one identity record with equal placement keys
+//     is the motion (motion-node) trace_triangles / trace_paths on its mesh, and with equal vertex keys a deforming
+//     bottom is the static bottom on its tree;
+//   * errors, workspace, streams, n == 0 and the host build are the motion forms', the messages naming
+//     "trace_instances (deforming)" or "trace_instance_paths (deforming)";
+//   * the kernels are the instance kernels with the shader wrapped as detail::MotionShader<T,
+//     detail::WithDeformingBottoms<T, Shader>>: an if constexpr on detail::IsDeforming picks, per record, the motion
+//     inner step or the plain one and the key leaf (detail::deforming_instance_leaf) or instance_leaf.  The float kernels
+//     stay at 56 registers and spill (DESIGN.md section 6).
+// One frame (INTEGRATION.md §5 has it whole):
+//
+//     skin<<<...>>>(d_key0, d_key1);                                   // yours: the character's vertex keys
+//     prepare_motion_nodes(character, mesh, d_motion_nodes, bottom_up, character.bottom_up_workspace_bytes(), stream);
+//     write_keys<<<...>>>(d_recs, open, close);                        // yours: every record's placement keys
+//     prepare_deforming_instances(DeformingInstances<float> { d_recs, count, max_depth }, d_boxes, d_centres, stream);
+//     bvh3f_refit_boxes(top_bvh, d_boxes, count, BVH_DEVICE_POINTERS);
+//     top.trace_instances<false, false>(n, DeformingInstances<float> { d_recs, count, max_depth }, Shade { ... }, workspace, bytes, stream);
+//
 // Stacks: anything with push(Index) and try_pop(Index&) (false when empty), empty at the start.  A traversal holds at
 // most view.stack_bound() = depth + 1 entries, and no stack checks its capacity on the device: check it on the host
 // (DeviceView<T>::from(c, capacity) and bvh::v2::cuda::Accel<T>::device_view(capacity) throw when it is too small).
@@ -708,6 +744,35 @@ template <typename T> struct MotionNodes {
     size_t node_count = 0;
 };
 
+// One placed copy of a mesh in a scene that mixes bottom kinds, for the deforming forms of trace_instances and
+// trace_instance_paths: MotionInstance<T>'s fields (the bottom view's arrays, root, depth and the two placement keys,
+// in the same layout), then the bottom's vertex keys and motion nodes.  Each record picks its bottom kind:
+//   * vertices[0] == nullptr: a static bottom, the view's tris and node bounds, as in MotionInstance<T>;
+//   * vertices set, motion_nodes == nullptr: a deforming bottom on shutter boxes, triangle_at(vertices, id, time) under
+//     the view's tree (refitted over prepare_motion_triangles' boxes);
+//   * both set: a deforming bottom with motion nodes, whose inner steps are motion_inner_step at the ray's time (the
+//     view's node bounds are not read).
+// vertices[k] is the MotionTriangles<T> layout (count x 9 values in original order).  Fill it with
+// make_deforming_instance; root_index is written by prepare_deforming_instances.  160 bytes in float, 256 in double.
+template <typename T> struct alignas(16) DeformingInstance {
+    const bvhb200::DevNode<T>* nodes;   // the bottom view's nodes, prim_ids (BVH order) and tris (BVH order; static bottoms)
+    const uint32_t* prim_ids;
+    const bvhb200::DevTri<T>* tris;
+    typename bvhb200::Real<T>::UInt root_index;     // the bottom root's index, written by prepare_deforming_instances
+    uint32_t depth;                     // the bottom tree's depth
+    T object_to_world[2][12];           // the placement keys at time 0 and time 1, as in MotionInstance<T>
+    const T* vertices[2];               // the bottom's vertex keys at time 0 and time 1, or nullptr (a static bottom)
+    const MotionNode<T>* motion_nodes;  // the bottom's motion nodes (view.node_count + 1 records), or nullptr
+};
+static_assert(sizeof(DeformingInstance<float>) == 160 && sizeof(DeformingInstance<double>) == 256, "deforming instance size");
+
+// A plain view of `count` deforming-scene records in device memory; max_depth as in Instances<T>.
+template <typename T> struct DeformingInstances {
+    DeformingInstance<T>* records = nullptr;
+    size_t count = 0;
+    size_t max_depth = 0;
+};
+
 namespace detail {
 template <typename T> struct ViewTypes;
 template <> struct ViewTypes<float>  {
@@ -786,9 +851,15 @@ BVH_HD void shader_leaf(const TriangleShader<T, Shader>& ts, Payload& payload, u
                                return static_cast<bool>(ts.shader.accept(payload, static_cast<size_t>(ts.prim_ids[slot]), t, u, v));
                            });
 }
-// The record kind of a shader: Instance<T>, or MotionInstance<T> under a MotionShader.
+// The caller's shader of the deforming forms of trace_instances and trace_instance_paths; defined below.
+template <typename T, typename Shader> struct WithDeformingBottoms;
+// The record kind of a shader: Instance<T>, MotionInstance<T> under a MotionShader, or DeformingInstance<T> under a
+// MotionShader of WithDeformingBottoms.
 template <typename T, typename Shader> struct RecordOf { using type = Instance<T>; };
 template <typename T, typename Shader> struct RecordOf<T, MotionShader<T, Shader>> { using type = MotionInstance<T>; };
+template <typename T, typename Shader> struct RecordOf<T, MotionShader<T, WithDeformingBottoms<T, Shader>>> {
+    using type = DeformingInstance<T>;
+};
 
 // What the kernel of DeviceView::trace_instances reads besides the top tree's nodes: the caller's shader, the instance
 // records and the top tree's prim_ids (BVH-order slot -> record).
@@ -1224,21 +1295,34 @@ template <typename T> struct MotionNodeBuilder {
 //   * so each side of the union is moved out by a further 3 eps (S0_i + S1_i) + the smallest normal number: the
 //     margin beyond 1.5 eps covers the rounding of that widening (at most eps/2 of a bound below S0_i + S1_i).
 // A key with a non-finite entry gives the empty box and a zero centre: no ray reaches the record.
+// (shutter_keys_finite and shutter_world_box, `ok` its result, are that box; prepare_deforming_instance uses them too.
+// The root index is written between them, in the order this function always had.)
+template <typename T> BVH_HD bool shutter_keys_finite(const T (&keys)[2][12]);
+template <typename T>
+BVH_HD void shutter_world_box(const T (&keys)[2][12], const T* rb, bool ok, typename ViewTypes<T>::BBox& box, typename ViewTypes<T>::Vec& centre);
 template <typename T>
 BVH_HD void prepare_motion_instance(MotionInstance<T>& rec, typename ViewTypes<T>::BBox& box, typename ViewTypes<T>::Vec& centre) {
+    const bool ok = shutter_keys_finite(rec.object_to_world);
+    rec.root_index = rec.nodes[1].index;
+    shutter_world_box(rec.object_to_world, rec.nodes[1].bounds, ok, box, centre);
+}
+template <typename T> BVH_HD bool shutter_keys_finite(const T (&keys)[2][12]) {
+    using R = bvhb200::Real<T>;
+    bool ok = true;
+    for (int k = 0; k < 12; ++k) ok = ok && R::is_finite(keys[0][k]) && R::is_finite(keys[1][k]);
+    return ok;
+}
+template <typename T>
+BVH_HD void shutter_world_box(const T (&keys)[2][12], const T* rb, bool ok, typename ViewTypes<T>::BBox& box, typename ViewTypes<T>::Vec& centre) {
     using R = bvhb200::Real<T>;
     using UI = typename R::UInt;
     const T inf = R::from_bits(sizeof(T) == 4 ? (UI)0x7F800000u : (UI)0x7FF0000000000000ull);
     const T pad = R::mul(R::eps(), T(3)), tiny = sizeof(T) == 4 ? (T)FLT_MIN : (T)DBL_MIN;
-    bool ok = true;
-    for (int k = 0; k < 12; ++k) ok = ok && R::is_finite(rec.object_to_world[0][k]) && R::is_finite(rec.object_to_world[1][k]);
-    rec.root_index = rec.nodes[1].index;
-    const T* rb = rec.nodes[1].bounds;
     T lo[3], hi[3], mid[3];
     for (int i = 0; i < 3; ++i) {
         T lo0, hi0, s0, lo1, hi1, s1;
-        world_box_axis(rec.object_to_world[0], rb, i, lo0, hi0, s0);
-        world_box_axis(rec.object_to_world[1], rb, i, lo1, hi1, s1);
+        world_box_axis(keys[0], rb, i, lo0, hi0, s0);
+        world_box_axis(keys[1], rb, i, lo1, hi1, s1);
         const T d = R::add(R::mul(R::add(s0, s1), pad), tiny);
         lo[i] = R::sub(lo1 < lo0 ? lo1 : lo0, d);
         hi[i] = R::add(hi0 < hi1 ? hi1 : hi0, d);
@@ -1251,6 +1335,40 @@ BVH_HD void prepare_motion_instance(MotionInstance<T>& rec, typename ViewTypes<T
     box.min.x = lo[0]; box.min.y = lo[1]; box.min.z = lo[2];
     box.max.x = hi[0]; box.max.y = hi[1]; box.max.z = hi[2];
     centre.x = mid[0]; centre.y = mid[1]; centre.z = mid[2];
+}
+
+// prepare_deforming_instances for one record (both builds): prepare_motion_instance's box (shutter_world_box) of a
+// bottom box B that holds every finite triangle of the bottom at every time, and the root index.
+//   * static and shutter-box bottoms: B is the view's root box.  A static bottom's box holds its triangles; a
+//     shutter-box bottom's tree is refitted over prepare_motion_triangles' boxes, each of which holds triangle_at at
+//     every time (detail::prepare_motion_triangle);
+//   * motion-node bottoms: B is the union of the root motion node's two key boxes, and root_index is the root motion
+//     node's index.  Every coordinate of triangle_at(tris, id, tau) lies in it: in exact arithmetic the blend lies
+//     between the coordinate's two keys, each inside the unwidened key box of its leaf; blend_key rounds it by at most
+//     1.5 eps M (1 + O(eps)), M the largest magnitude of the leaf's bounds on that axis, and a leaf side on an axis on
+//     which anything moves is widened by 4 eps M + the smallest normal number (MotionNodeBuilder), of which the
+//     rounding of the widening takes back at most eps/2 (M + d).  On an axis on which nothing moves the blend is the key
+//     itself.  Inner keys are unions of their children's (and possibly widened further), so the root's keys hold every
+//     leaf's.  (node_at at some time is not used: its own blend can round one ulp inside a key, which the union
+//     of the keys never does.)
+// A triangle with a non-finite key is in no box (prepare_motion_triangles and prepare_motion_nodes leave it out).
+template <typename T>
+BVH_HD void prepare_deforming_instance(DeformingInstance<T>& rec, typename ViewTypes<T>::BBox& box, typename ViewTypes<T>::Vec& centre) {
+    if (rec.vertices[0] && rec.motion_nodes) {
+        const MotionNode<T>& root = rec.motion_nodes[1];
+        T rb[6];
+        for (int a = 0; a < 2; ++a) {
+            rb[2 * a] = root.xy[1][2 * a] < root.xy[0][2 * a] ? root.xy[1][2 * a] : root.xy[0][2 * a];
+            rb[2 * a + 1] = root.xy[0][2 * a + 1] < root.xy[1][2 * a + 1] ? root.xy[1][2 * a + 1] : root.xy[0][2 * a + 1];
+        }
+        rb[4] = root.z[1][0] < root.z[0][0] ? root.z[1][0] : root.z[0][0];
+        rb[5] = root.z[0][1] < root.z[1][1] ? root.z[1][1] : root.z[0][1];
+        rec.root_index = root.index;
+        shutter_world_box(rec.object_to_world, rb, shutter_keys_finite(rec.object_to_world), box, centre);
+    } else {
+        rec.root_index = rec.nodes[1].index;
+        shutter_world_box(rec.object_to_world, rec.nodes[1].bounds, shutter_keys_finite(rec.object_to_world), box, centre);
+    }
 }
 
 // The triangle leaf of trace_instances (both builds): the library's leaf_range over [first, first + count) of instance
@@ -1337,6 +1455,58 @@ template <typename T, typename Shader> struct WithMotionNodes {
 template <typename Shader> struct HasMotionNodes : std::false_type {};
 template <typename T, typename Shader> struct HasMotionNodes<MotionShader<T, WithMotionNodes<T, Shader>>> : std::true_type {};
 
+// The caller's shader of the deforming forms of trace_instances and trace_instance_paths.  It runs wrapped in
+// MotionShader, like the shader of the motion forms (so the time, the placement at that time and the record are
+// theirs); the instance kernels see it through IsDeforming, read DeformingInstance<T> records and pick each record's
+// bottom kind at run time.
+template <typename T, typename Shader> struct WithDeformingBottoms {
+    using Payload = typename Shader::Payload;
+    Shader shader;
+    template <typename... A> BVH_HD decltype(auto) start(A&&... a) const { return shader.start(std::forward<A>(a)...); }
+    template <typename... A> BVH_HD decltype(auto) accept(A&&... a) const { return shader.accept(std::forward<A>(a)...); }
+    template <typename... A> BVH_HD decltype(auto) next(A&&... a) const { return shader.next(std::forward<A>(a)...); }
+    template <typename... A> BVH_HD void finish(A&&... a) const { shader.finish(std::forward<A>(a)...); }
+};
+// Whether an instance kernel's shader runs DeformingInstance<T> records
+template <typename Shader> struct IsDeforming : std::false_type {};
+template <typename T, typename Shader> struct IsDeforming<MotionShader<T, WithDeformingBottoms<T, Shader>>> : std::true_type {};
+
+// The triangle leaf of a deforming bottom (both builds): instance_leaf with the triangles built at the payload's time.
+// Per slot: the original id, triangle_at from the record's vertex keys, precompute_tri and the library's tri_test
+// without its own tie rule; the filter applies instance_leaf's canonical rule on (instance, original id), then the
+// shader's accept, and notes the instance of an accepted hit.  Not unrolled, as the motion forms' leaf.
+template <typename T, bool TieLastVisited, typename Shader, typename Payload>
+BVH_HD void deforming_instance_leaf(const Shader& shader, const DeformingInstance<T>& rec, uint32_t inst, Payload& payload, uint32_t first,
+                                    uint32_t count, bvhb200::RayCtx<T>& r, bvhb200::HitState<T>& hit, uint32_t& hit_inst) {
+    const MotionTriangles<T> tris { { rec.vertices[0], rec.vertices[1] }, 0 };
+    const uint32_t* ids = rec.prim_ids;
+#if defined(__CUDA_ARCH__)
+    #pragma unroll 1
+#endif
+    for (uint32_t slot = first; slot < first + count; ++slot) {
+        const uint32_t id = ids[slot];
+        T v[9];
+        triangle_at(tris, id, payload.time, v);
+        const bvhb200::DevTri<T> tri = bvhb200::precompute_tri(v);
+        bvhb200::tri_test<T>(tri, slot, ids, false, r, hit, [&](uint32_t, T t, T u, T w) {
+            if (!TieLastVisited && hit.slot != bvhb200::kInvalidId && !(t < hit.t)) {  // an exact tie with the current best
+                if (inst != hit_inst ? inst > hit_inst : !(id < ids[hit.slot])) return false;
+            }
+            if (!static_cast<bool>(shader.accept(payload, inst, static_cast<size_t>(id), t, u, w))) return false;
+            hit_inst = inst;
+            return true;
+        });
+    }
+}
+// The leaf phase of a deforming-scene record (both builds): deforming_instance_leaf when it has vertex keys, otherwise
+// instance_leaf on the view's triangles.
+template <typename T, bool TieLastVisited, typename Shader, typename Payload>
+BVH_HD void deforming_bottom_leaf(const Shader& shader, const DeformingInstance<T>& rec, uint32_t inst, Payload& payload, uint32_t first,
+                                  uint32_t count, bvhb200::RayCtx<T>& r, bvhb200::HitState<T>& hit, uint32_t& hit_inst) {
+    if (rec.vertices[0]) deforming_instance_leaf<T, TieLastVisited>(shader, rec, inst, payload, first, count, r, hit, hit_inst);
+    else instance_leaf<T, TieLastVisited>(shader, rec.tris, rec.prim_ids, inst, payload, first, count, r, hit, hit_inst);
+}
+
 // The inner step of the motion-node forms (both builds): inner_step with each child's box blended to the ray's time.
 // Per child, node_at's blend (blend_node_xy, blend_node_z) at tau = shutter_time(time), then node_test's slab arithmetic
 // and descend, unchanged.  Float closest-hit rays split the fetch as inner_step does: x and y of both keys of both
@@ -1376,8 +1546,14 @@ BVH_HD void motion_inner_step(const MotionNode<T>* __restrict__ nodes, T time, c
 // a motion record, the inverse of blend_keys at the payload's time (instance_at's), built here.  All NaN: no inverse.
 template <typename T, typename Payload, typename F>
 BVH_HD void with_world_to_object(const Instance<T>& rec, const Payload&, F&& f) { f(static_cast<const T*>(rec.world_to_object)); }
-template <typename T, typename Payload, typename F>
-BVH_HD void with_world_to_object(const MotionInstance<T>& rec, const Payload& payload, F&& f) {
+// The records whose placement moves over the shutter, both keys in object_to_world[2][12]: MotionInstance<T> and
+// DeformingInstance<T>
+template <typename Rec> struct MotionRecord : std::false_type {};
+template <typename T> struct MotionRecord<MotionInstance<T>> : std::true_type { using Scalar = T; };
+template <typename T> struct MotionRecord<DeformingInstance<T>> : std::true_type { using Scalar = T; };
+template <typename Rec, typename Payload, typename F, std::enable_if_t<MotionRecord<Rec>::value, int> = 0>
+BVH_HD void with_world_to_object(const Rec& rec, const Payload& payload, F&& f) {
+    using T = typename MotionRecord<Rec>::Scalar;
     T m[12], inv[12];
     blend_keys(rec.object_to_world, payload.time, m);
     invert_affine(m, inv);
@@ -1385,13 +1561,15 @@ BVH_HD void with_world_to_object(const MotionInstance<T>& rec, const Payload& pa
 }
 }
 
-// The placement of motion record `rec` at `time` (both builds): the Instance<T> the motion forms of trace_instances and
-// trace_instance_paths trace a ray of that time through.  Its object_to_world is the blend of the keys
-// (detail::blend_keys: time clamped to [0, 1], a NaN time as 0; exact at 0 and 1 and for coefficients that do not
-// move), its world_to_object prepare_instance's inverse of that (all NaN when it has none: the ray skips the record),
-// and root_index, depth and the bottom arrays are the record's.
-template <typename T> BVH_HD Instance<T> instance_at(const MotionInstance<T>& rec, T time) {
-    Instance<T> out;
+// The placement of motion record `rec` (MotionInstance<T> or DeformingInstance<T>) at `time` (both builds): the
+// Instance<T> the motion and deforming forms of trace_instances and trace_instance_paths trace a ray of that time
+// through.  Its object_to_world is the blend of the keys (detail::blend_keys: time clamped to [0, 1], a NaN time as 0;
+// exact at 0 and 1 and for coefficients that do not move), its world_to_object prepare_instance's inverse of that (all
+// NaN when it has none: the ray skips the record), and root_index, depth and the bottom arrays are the record's.  (A
+// deforming bottom's triangles at that time are triangle_at of the record's vertex keys, not these arrays' tris.)
+template <typename Rec, std::enable_if_t<detail::MotionRecord<Rec>::value, int> = 0>
+BVH_HD Instance<typename detail::MotionRecord<Rec>::Scalar> instance_at(const Rec& rec, typename detail::MotionRecord<Rec>::Scalar time) {
+    Instance<typename detail::MotionRecord<Rec>::Scalar> out;
     out.nodes = rec.nodes; out.prim_ids = rec.prim_ids; out.tris = rec.tris;
     out.root_index = rec.root_index;
     out.depth = rec.depth;
@@ -1508,10 +1686,10 @@ __device__ __forceinline__ void enter_instance(const InstanceShader<T, Shader>& 
     inst = id;
     top = rec->root_index;
 }
-// enter_motion_instance: enter_instance for motion records: the placement at the time in the lane's payload is built
-// first (with_world_to_object), and the instance is skipped when it has no inverse at that time.  A separate function
-// rather than a form of enter_instance: every shared form tried changed the register assignment of
-// device_view_instance_kernel for static records (DESIGN.md section 8).
+// enter_motion_instance: enter_instance for motion records (MotionInstance<T> or DeformingInstance<T>): the placement
+// at the time in the lane's payload is built first (with_world_to_object), and the instance is skipped when it has no
+// inverse at that time.  A separate function rather than a form of enter_instance: every shared form tried changed the
+// register assignment of device_view_instance_kernel for static records (DESIGN.md section 8).
 template <typename T, bool IsRobust, typename U, typename Shader, typename Payload>
 __device__ __forceinline__ void enter_motion_instance(const InstanceShader<T, Shader>& is, const Payload& payload,
                                                       bvhb200::SmemStack<U>& stack, bvhb200::RayCtx<T>& r, uint32_t& inst, U& top) {
@@ -1519,7 +1697,7 @@ __device__ __forceinline__ void enter_motion_instance(const InstanceShader<T, Sh
     const U first = bvhb200::index_first(top);
     const uint32_t count = bvhb200::index_count(top);
     const uint32_t id = is.prim_ids[first];
-    const MotionInstance<T>* rec = is.records + id;
+    const auto* rec = is.records + id;
     const U rest = bvhb200::make_index<U>(first + 1, count - 1);
     with_world_to_object(*rec, payload, [&](const T* world_to_object) {
         if (instance_is_singular(world_to_object)) {
@@ -1910,14 +2088,23 @@ device_view_instance_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsig
     };
 
     // inner phase: descend the current level until this lane holds a leaf or the marker, its ray is finished, or the step
-    // budget of this round is spent
+    // budget of this round is spent (in a deforming scene, a bottom with motion nodes takes their boxes at the ray's time)
     auto inner = [&] {
         if (has_ray) {
             const bvhb200::DevNode<T>* level = inst == detail::kNoInstance ? nodes : is.records[inst].nodes;
             uint32_t budget = inner_budget;
-            while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone and the marker end it too)
-                --budget;
-                bvhb200::inner_step<T, IsAnyHit, IsRobust>(level, r, top, stack);
+            if constexpr (detail::IsDeforming<Shader>::value) {
+                const MotionNode<T>* motion_nodes = inst == detail::kNoInstance ? nullptr : is.records[inst].motion_nodes;
+                while (bvhb200::index_count(top) == 0 && budget != 0) {
+                    --budget;
+                    if (motion_nodes) detail::motion_inner_step<T, IsAnyHit, IsRobust>(motion_nodes, payload.time, r, top, stack);
+                    else bvhb200::inner_step<T, IsAnyHit, IsRobust>(level, r, top, stack);
+                }
+            } else {
+                while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone and the marker end it too)
+                    --budget;
+                    bvhb200::inner_step<T, IsAnyHit, IsRobust>(level, r, top, stack);
+                }
             }
             if (top == kDone) retire();
         }
@@ -1937,8 +2124,12 @@ device_view_instance_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, unsig
         if (!has_ray || bvhb200::index_count(top) == 0) return;
         if (inst != detail::kNoInstance && top != kMarker) {
             const auto* rec = is.records + inst;
-            detail::instance_leaf<T, TieLastVisited>(is.shader, rec->tris, rec->prim_ids, inst, payload, (uint32_t)bvhb200::index_first(top),
-                                                     bvhb200::index_count(top), r, hit, hit_inst);
+            if constexpr (detail::IsDeforming<Shader>::value)
+                detail::deforming_bottom_leaf<T, TieLastVisited>(is.shader, *rec, inst, payload, (uint32_t)bvhb200::index_first(top),
+                                                                 bvhb200::index_count(top), r, hit, hit_inst);
+            else
+                detail::instance_leaf<T, TieLastVisited>(is.shader, rec->tris, rec->prim_ids, inst, payload, (uint32_t)bvhb200::index_first(top),
+                                                         bvhb200::index_count(top), r, hit, hit_inst);
             if (IsAnyHit && hit.slot != bvhb200::kInvalidId) { retire(); return; }
             top = bvhb200::pop_or_done<U>(stack);                  // (the marker at the latest)
         }
@@ -2031,10 +2222,24 @@ device_view_instance_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, 
         if (has_path) {
             const bvhb200::DevNode<T>* level = inst == detail::kNoInstance ? nodes : is.records[inst].nodes;
             uint32_t budget = inner_budget;
-            while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone and the marker end it too)
-                --budget;
-                if (occlusion) bvhb200::inner_step<T, true, IsRobust>(level, r, top, stack);
-                else bvhb200::inner_step<T, false, IsRobust>(level, r, top, stack);
+            if constexpr (detail::IsDeforming<Shader>::value) {       // (device_view_instance_kernel's choice per record)
+                const MotionNode<T>* motion_nodes = inst == detail::kNoInstance ? nullptr : is.records[inst].motion_nodes;
+                while (bvhb200::index_count(top) == 0 && budget != 0) {
+                    --budget;
+                    if (motion_nodes) {
+                        if (occlusion) detail::motion_inner_step<T, true, IsRobust>(motion_nodes, payload.time, r, top, stack);
+                        else detail::motion_inner_step<T, false, IsRobust>(motion_nodes, payload.time, r, top, stack);
+                    } else {
+                        if (occlusion) bvhb200::inner_step<T, true, IsRobust>(level, r, top, stack);
+                        else bvhb200::inner_step<T, false, IsRobust>(level, r, top, stack);
+                    }
+                }
+            } else {
+                while (bvhb200::index_count(top) == 0 && budget != 0) {     // (kTraversalDone and the marker end it too)
+                    --budget;
+                    if (occlusion) bvhb200::inner_step<T, true, IsRobust>(level, r, top, stack);
+                    else bvhb200::inner_step<T, false, IsRobust>(level, r, top, stack);
+                }
             }
         }
     };
@@ -2051,8 +2256,12 @@ device_view_instance_path_kernel(const bvhb200::DevNode<T>* __restrict__ nodes, 
         if (!has_path || bvhb200::index_count(top) == 0) return;
         if (inst != detail::kNoInstance && top != kMarker) {
             const auto* rec = is.records + inst;
-            detail::instance_leaf<T, TieLastVisited>(is.shader, rec->tris, rec->prim_ids, inst, payload, (uint32_t)bvhb200::index_first(top),
-                                                     bvhb200::index_count(top), r, hit, hit_inst);
+            if constexpr (detail::IsDeforming<Shader>::value)
+                detail::deforming_bottom_leaf<T, TieLastVisited>(is.shader, *rec, inst, payload, (uint32_t)bvhb200::index_first(top),
+                                                                 bvhb200::index_count(top), r, hit, hit_inst);
+            else
+                detail::instance_leaf<T, TieLastVisited>(is.shader, rec->tris, rec->prim_ids, inst, payload, (uint32_t)bvhb200::index_first(top),
+                                                         bvhb200::index_count(top), r, hit, hit_inst);
             if (occlusion && hit.slot != bvhb200::kInvalidId) { end_segment(); return; }
             top = bvhb200::pop_or_done<U>(stack);                  // (the marker at the latest)
         }
@@ -2077,6 +2286,14 @@ __global__ void prepare_motion_instances_kernel(MotionInstance<T>* records, size
                                                 typename detail::ViewTypes<T>::Vec* centers) {
     const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i < count) detail::prepare_motion_instance<T>(records[i], bboxes[i], centers[i]);
+}
+
+// The kernel of prepare_deforming_instances: one thread per record.
+template <typename T>
+__global__ void prepare_deforming_instances_kernel(DeformingInstance<T>* records, size_t count, typename detail::ViewTypes<T>::BBox* bboxes,
+                                                   typename detail::ViewTypes<T>::Vec* centers) {
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i < count) detail::prepare_deforming_instance<T>(records[i], bboxes[i], centers[i]);
 }
 
 // The kernel of prepare_motion_triangles: one thread per triangle.
@@ -2452,6 +2669,40 @@ template <typename T> struct DeviceView {
                                                       workspace, workspace_bytes, on_stream);
     }
 
+    // The same through a scene that mixes static and deforming bottoms under moving placements, each ray at its own
+    // time: see "Deforming instances" at the top of this file.  The shader is a motion form's (start also gives the time).
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instances(size_t n, const DeformingInstances<T>& instances, const Shader& shader, void* workspace,
+                         size_t workspace_bytes) const {
+        trace_instances<IsAnyHit, IsRobust, TieLastVisited>(n, instances, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsAnyHit, bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instances(size_t n, const DeformingInstances<T>& instances, const Shader& shader, void* workspace, size_t workspace_bytes,
+                         void* on_stream) const {
+        using MS = detail::MotionShader<T, detail::WithDeformingBottoms<T, Shader>>;
+        instance_batch<IsAnyHit, IsRobust, TieLastVisited>(
+            "trace_instances (deforming)", n, instances,
+            detail::InstanceShader<T, MS> { MS { detail::WithDeformingBottoms<T, Shader> { shader } }, instances.records, prim_ids },
+            workspace, workspace_bytes, on_stream);
+    }
+    // Whole paths through such a scene, each path at its own time.
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instance_paths(size_t n, const DeformingInstances<T>& instances, const Shader& shader, void* workspace,
+                              size_t workspace_bytes) const {
+        trace_instance_paths<IsRobust, TieLastVisited>(n, instances, shader, workspace, workspace_bytes, stream);
+    }
+    // `on_stream` is a cudaStream_t (unused by the host pass)
+    template <bool IsRobust, bool TieLastVisited = false, typename Shader>
+    void trace_instance_paths(size_t n, const DeformingInstances<T>& instances, const Shader& shader, void* workspace,
+                              size_t workspace_bytes, void* on_stream) const {
+        using MS = detail::MotionShader<T, detail::WithDeformingBottoms<T, Shader>>;
+        instance_path_batch<IsRobust, TieLastVisited>(
+            "trace_instance_paths (deforming)", n, instances,
+            detail::InstanceShader<T, MS> { MS { detail::WithDeformingBottoms<T, Shader> { shader } }, instances.records, prim_ids },
+            workspace, workspace_bytes, on_stream);
+    }
+
     // PrecomputedTri::intersect (reference tri.h:55-74) on BVH-order triangle k: true, with the hit's distance and
     // barycentrics, when the ray meets it at a distance in [ray.tmin, ray.tmax].  The batched kernels' own test.
     BVH_HD bool intersect_tri(size_t k, const Ray& ray, T& t, T& u, T& v) const {
@@ -2675,14 +2926,40 @@ private:
                         bvhb200::ray_prologue<T, IsRobust>(o);
                         detail::VectorStack<Index> bottom;
                         bottom.elems.reserve(rec.depth + 1);
-                        bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
-                            rec.nodes, o, rec.root_index, bottom,
-                            [&](Index b, Index e) {
-                                detail::instance_leaf<T, TieLastVisited>(is.shader, rec.tris, rec.prim_ids, id, payload, (uint32_t)b,
-                                                                         (uint32_t)(e - b), o, hit, hit_inst);
-                                return hit.slot != bvhb200::kInvalidId;
-                            },
-                            [](Index) {});
+                        if constexpr (detail::IsDeforming<Shader>::value) {
+                            // the record's bottom kind: the leaf of deforming_bottom_leaf, and with motion nodes
+                            // traverse_top_down's loop with their inner step (host_triangle_ray's)
+                            if (rec.motion_nodes) {
+                                Index top = rec.root_index;
+                                for (;;) {
+                                    while (bvhb200::index_count(top) == 0)
+                                        detail::motion_inner_step<T, IsAnyHit, IsRobust>(rec.motion_nodes, payload.time, o, top, bottom);
+                                    if (top == bvhb200::kTraversalDone<Index>) break;
+                                    detail::deforming_bottom_leaf<T, TieLastVisited>(is.shader, rec, id, payload, (uint32_t)bvhb200::index_first(top),
+                                                                                     bvhb200::index_count(top), o, hit, hit_inst);
+                                    if (IsAnyHit && hit.slot != bvhb200::kInvalidId) break;
+                                    top = bvhb200::pop_or_done<Index>(bottom);
+                                }
+                            } else {
+                                bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
+                                    rec.nodes, o, rec.root_index, bottom,
+                                    [&](Index b, Index e) {
+                                        detail::deforming_bottom_leaf<T, TieLastVisited>(is.shader, rec, id, payload, (uint32_t)b,
+                                                                                         (uint32_t)(e - b), o, hit, hit_inst);
+                                        return hit.slot != bvhb200::kInvalidId;
+                                    },
+                                    [](Index) {});
+                            }
+                        } else {
+                            bvhb200::traverse_top_down<T, IsAnyHit, IsRobust>(
+                                rec.nodes, o, rec.root_index, bottom,
+                                [&](Index b, Index e) {
+                                    detail::instance_leaf<T, TieLastVisited>(is.shader, rec.tris, rec.prim_ids, id, payload, (uint32_t)b,
+                                                                             (uint32_t)(e - b), o, hit, hit_inst);
+                                    return hit.slot != bvhb200::kInvalidId;
+                                },
+                                [](Index) {});
+                        }
                         r.tmax = o.tmax;
                         if (IsAnyHit && hit.slot != bvhb200::kInvalidId) return true;
                     }
@@ -2838,6 +3115,86 @@ void prepare_motion_instances(const MotionInstances<T>& instances, typename deta
 #else
     (void)stream;
     for (size_t i = 0; i < instances.count; ++i) detail::prepare_motion_instance<T>(instances.records[i], bboxes[i], centers[i]);
+#endif
+}
+
+// A deforming-scene record of the mesh `view` placed by `key0` at time 0 and `key1` at time 1 (12 values each, 3 x 4
+// row-major), on the host.  Without motion_tris the bottom is static (the view must have triangles); with them it
+// deforms, on the view's tree refitted over prepare_motion_triangles' boxes or, with motion_nodes, on those nodes (the
+// view needs no triangles).  Throws std::invalid_argument for a static bottom whose view has no triangles, null keys
+// or motion nodes, motion_tris.count other than view.prim_count or motion_nodes.node_count other than
+// view.node_count.  root_index is 0 until
+// prepare_deforming_instances writes it.
+namespace detail {
+// make_deforming_instance's record of `view` under the keys, before its bottom kind is set (a static bottom)
+template <typename T> DeformingInstance<T> deforming_record(const DeviceView<T>& view, const T* key0, const T* key1) {
+    DeformingInstance<T> rec;
+    rec.nodes = view.nodes; rec.prim_ids = view.prim_ids; rec.tris = view.tris;
+    rec.root_index = 0;
+    rec.depth = static_cast<uint32_t>(view.depth);
+    for (int k = 0; k < 12; ++k) {
+        rec.object_to_world[0][k] = key0[k];
+        rec.object_to_world[1][k] = key1[k];
+    }
+    rec.vertices[0] = rec.vertices[1] = nullptr;
+    rec.motion_nodes = nullptr;
+    return rec;
+}
+}
+template <typename T> DeformingInstance<T> make_deforming_instance(const DeviceView<T>& view, const T* key0, const T* key1) {
+    if (!view.tris)
+        throw std::invalid_argument("bvh::v2::cuda::make_deforming_instance: a static bottom needs a view with triangles (built from boxes)");
+    return detail::deforming_record(view, key0, key1);
+}
+template <typename T>
+DeformingInstance<T> make_deforming_instance(const DeviceView<T>& view, const T* key0, const T* key1, const MotionTriangles<T>& motion_tris) {
+    const std::string who = "bvh::v2::cuda::make_deforming_instance: ";
+    if (!motion_tris.vertices[0] || !motion_tris.vertices[1]) throw std::invalid_argument(who + "a null vertex key");
+    if (motion_tris.count != view.prim_count)
+        throw std::invalid_argument(who + std::to_string(motion_tris.count) + " triangles for a tree of " + std::to_string(view.prim_count) +
+                                    " primitives");
+    DeformingInstance<T> rec = detail::deforming_record(view, key0, key1);
+    rec.vertices[0] = motion_tris.vertices[0];
+    rec.vertices[1] = motion_tris.vertices[1];
+    return rec;
+}
+template <typename T>
+DeformingInstance<T> make_deforming_instance(const DeviceView<T>& view, const T* key0, const T* key1, const MotionTriangles<T>& motion_tris,
+                                             const MotionNodes<T>& motion_nodes) {
+    const std::string who = "bvh::v2::cuda::make_deforming_instance: ";
+    if (!motion_nodes.nodes) throw std::invalid_argument(who + "a null motion-node pointer");
+    if (motion_nodes.node_count != view.node_count)
+        throw std::invalid_argument(who + "motion nodes of " + std::to_string(motion_nodes.node_count) + " nodes for a tree of " +
+                                    std::to_string(view.node_count) + " nodes");
+    DeformingInstance<T> rec = make_deforming_instance(view, key0, key1, motion_tris);
+    rec.motion_nodes = motion_nodes.nodes;
+    return rec;
+}
+
+// prepare_motion_instances for deforming-scene records (one thread each, stream-ordered on `stream`, no host
+// synchronisation): every root index (the root motion node's for a bottom with motion nodes, otherwise the view's), and
+// in bboxes[i] / centers[i] a world box that holds every finite triangle of record i's bottom at every time of the
+// shutter under its placement at that time, and its centre, ready for bvhNN_build_boxes or bvhNN_refit_boxes with
+// BVH_DEVICE_POINTERS.  See detail::prepare_deforming_instance for the bottom box and the argument.  Each deforming
+// bottom's own step (prepare_motion_triangles and bvhNN_refit_boxes, or prepare_motion_nodes) must come first on the
+// stream.  The current device must be the records'.  A failed launch throws std::runtime_error.  Compiled as plain
+// host C++, the records are prepared serially in place.
+template <typename T>
+void prepare_deforming_instances(const DeformingInstances<T>& instances, typename detail::ViewTypes<T>::BBox* bboxes,
+                                 typename detail::ViewTypes<T>::Vec* centers, void* stream = nullptr) {
+    if (instances.count == 0) return;
+    if (!instances.records || !bboxes || !centers)
+        throw std::invalid_argument("bvh::v2::cuda::prepare_deforming_instances: null records, boxes or centres");
+#if defined(__CUDACC__)
+    const unsigned block = 128, grid = (unsigned)((instances.count + block - 1) / block);
+    prepare_deforming_instances_kernel<T><<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(instances.records, instances.count, bboxes,
+                                                                                              centers);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess)
+        throw std::runtime_error(std::string("bvh::v2::cuda::prepare_deforming_instances: launch: ") + cudaGetErrorString(e));
+#else
+    (void)stream;
+    for (size_t i = 0; i < instances.count; ++i) detail::prepare_deforming_instance<T>(instances.records[i], bboxes[i], centers[i]);
 #endif
 }
 
